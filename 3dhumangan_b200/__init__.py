@@ -1,4 +1,4 @@
-"""B200-native (sm_100a) implementation of the 3DHumanGAN generator/discriminator hot path.
+"""H100-native (sm_90a) implementation of the 3DHumanGAN generator/discriminator hot path.
 
 The directory name starts with a digit, so import it with
     pkg = importlib.import_module("3dhumangan_b200")

@@ -1,6 +1,6 @@
 """ctypes binding of the C ABI declared in include/hg3d.h.
 
-The product path has NO fallback: if `lib3dhg_sm100a.so` is missing, fails to load, or an entry
+The product path has NO fallback: if `lib3dhg_sm90a.so` is missing, fails to load, or an entry
 point returns non-zero, a RuntimeError is raised (mirroring TORCH_CHECK -> RuntimeError in the
 reference's own native ops, lib/components/ops/bias_act.cpp:34-51).  All pointers are raw device
 pointers taken from torch tensors; the library never allocates device memory and never
@@ -15,7 +15,7 @@ from ctypes import c_char_p, c_double, c_float, c_int, c_long, c_size_t, c_void_
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.path.join(_HERE, "lib3dhg_sm100a.so")
+LIB_PATH = os.path.join(_HERE, "lib3dhg_sm90a.so")
 _lib = None
 
 # name -> (restype, argtypes).  Keep in sync with include/hg3d.h (tests check every symbol).
@@ -153,7 +153,7 @@ _DEVICE_OK = set()
 
 def require_device(t=None):
     if not torch.cuda.is_available():
-        raise RuntimeError("hg3d: no CUDA device visible; the sm_100a kernels cannot run (no fallback)")
+        raise RuntimeError("hg3d: no CUDA device visible; the sm_90a kernels cannot run (no fallback)")
     dev = torch.cuda.current_device()
     if dev not in _DEVICE_OK:          # cudaGetDeviceProperties is slow: check each device once
         check(lib().hg_check_device(), "hg_check_device")
@@ -473,8 +473,9 @@ _WGH_WS = {}
 
 
 def _conv3x3_wgrad_halo(dy, x, passes):
-    """3x3 weight gradient on rows of >= 128 pixels (csrc/dconv_wgrad_halo.cu): per (128 output, 64 input)-channel block two
-    launches (5 + 4 taps, 8 x 64 TMEM columns at most), the input converted once per image row instead of once per tap."""
+    """3x3 weight gradient on rows of >= 128 pixels (csrc/dconv_wgrad_halo.cu): per (128 output, 64 input)-channel block three
+    launches (one filter row of 3 taps each: the accumulators of at most 4 taps fit the registers), the input converted once
+    per image row instead of once per tap."""
     B, Cout, H, W = dy.shape
     Cin = x.shape[1]
     dev = dy.device
@@ -483,7 +484,7 @@ def _conv3x3_wgrad_halo(dy, x, passes):
         ws = _WGH_WS[dev] = torch.empty(int(lib().hg_conv3x3_wgrad_halo_workspace_bytes()) // 4, dtype=torch.float32, device=dev)
     dW = torch.empty(Cout, Cin, 9, dtype=torch.float32, device=dev)
     db = torch.empty(Cout, dtype=torch.float32, device=dev)
-    groups = ([0, 1, 2, 3, 4], [5, 6, 7, 8])
+    groups = ([0, 1, 2], [3, 4, 5], [6, 7, 8])
     for co0 in range(0, Cout, 128):
         nco = min(128, Cout - co0)
         for ci0 in range(0, Cin, 64):
@@ -507,8 +508,8 @@ def _conv3x3_wgrad_halo(dy, x, passes):
 
 def conv2d_wgrad(dy, x, ksize, passes=3):
     """dW [Cout,Cin,k,k], dbias [Cout] of a stride-1 'same' convolution.  3x3 on rows of >= 128 pixels: the haloed kernel
-    (csrc/dconv_wgrad_halo.cu); otherwise csrc/dconv_bwd.cu: ONE launch per layer whose grid enumerates the (256 output,
-    256 input)-channel chunks and the groups of taps that fit the 512 TMEM columns (`hg_conv2d_wgrad_layer`; the per-group
+    (csrc/dconv_wgrad_halo.cu); otherwise csrc/dconv_bwd.cu: ONE launch per layer whose grid enumerates the (128 output,
+    256 input)-channel chunks and the groups of taps whose accumulators fit the registers (`hg_conv2d_wgrad_layer`; the per-group
     entry point `hg_conv2d_wgrad_taps` stays exported)."""
     B, Cout, H, W = dy.shape
     Cin = x.shape[1]

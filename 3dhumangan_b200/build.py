@@ -1,4 +1,4 @@
-"""Build lib3dhg_sm100a.so in-tree with nvcc (sm_100a only; no JIT cache, no fallback)."""
+"""Build lib3dhg_sm90a.so in-tree with nvcc (sm_90a only; no JIT cache, no fallback)."""
 from __future__ import annotations
 
 import glob
@@ -8,9 +8,9 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
-LIB = os.path.join(HERE, "lib3dhg_sm100a.so")
+LIB = os.path.join(HERE, "lib3dhg_sm90a.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC",
          "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
 
@@ -46,7 +46,7 @@ def build(force=False, verbose=False):
         failed |= rc != 0
     if failed:
         raise RuntimeError("nvcc failed (see messages above)")
-    subprocess.check_call([NVCC, "-shared", "-o", LIB, *objs, "-lcudart"])
+    subprocess.check_call([NVCC, "-shared", *FLAGS[:2], "-o", LIB, *objs, "-lcudart"])
     return LIB
 
 

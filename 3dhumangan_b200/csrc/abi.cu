@@ -20,7 +20,7 @@ const char* hg_last_error(void) { return hg::g_err; }
 
 int hg_abi_version(void) { return 1; }
 
-// Returns 0 when the current device is an sm_100 part this library was compiled for.
+// Returns 0 when the current device is an sm_90 part (H100 / H200) this library was compiled for.
 int hg_check_device(void) {
   int dev = 0;
   cudaDeviceProp p;
@@ -28,8 +28,8 @@ int hg_check_device(void) {
     hg::set_error("hg_check_device: no CUDA device");
     return 2;
   }
-  if (p.major != 10) {
-    hg::set_error("hg_check_device: device '%s' is sm_%d%d; this library contains sm_100a code only", p.name, p.major,
+  if (p.major != 9 || p.minor != 0) {
+    hg::set_error("hg_check_device: device '%s' is sm_%d%d; this library contains sm_90a code only", p.name, p.major,
                   p.minor);
     return 1;
   }

@@ -1,4 +1,4 @@
-// U-Net discriminator convolutions as implicit GEMMs on tcgen05.
+// U-Net discriminator convolutions as implicit GEMMs on wgmma.
 //
 // Replaces the cuDNN conv2d calls behind ResBlock / UNetDiscriminator
 // (lib/discriminators/unet_discriminators.py:7-72, 82-160): 3x3 (pad 1) and 1x1 convolutions over NCHW
@@ -7,17 +7,19 @@
 //   * nn.Upsample(scale_factor=2, nearest) in front (:26,41)    -> source pixel (y>>1, x>>1)
 //   * torch.cat((skip, x), dim=1) (:147)                        -> two source tensors, split by channel
 //   * bias, residual add `x_s + dx` (:54)                       -> epilogue
-// GEMM view: M = 128 consecutive output pixels of one image, N = Cout block (<= 256, up to two blocks),
-// K = taps x Cin in chunks of 64 (one tap, 64 channels); a 4-slot operand ring decouples the row warps
-// from the MMA thread.  Weights are pre-packed as [Cout, tap, Cin] (hg_pack_weight).
+// GEMM view: M = 128 consecutive output pixels of one image, N = one Cout block (<= 256 channels; a work item is one
+// pixel tile x one block, so that the [128 x 256] fp32 accumulator fits the registers of two warpgroups),
+// K = taps x Cin in chunks of 64 (one tap, 64 channels).  Warpgroup g (warps 4g..4g+3) builds rows 64g..64g+63 of each
+// operand chunk in a 4-slot ring and issues their wgmmas while it builds the next chunk; warp 8 streams the weight
+// tiles.  Weights are pre-packed as [Cout, tap, Cin] (hg_pack_weight).
 // AvgPool2d(2) of the down path is a separate streaming kernel (hg_pool_add).
 #include <stdlib.h>
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hg {
 
-constexpr int kDcThreads = 320;
+constexpr int kDcThreads = 384;   // warpgroups 0-1: operands + wgmma + epilogue, warp 8: weight stages
 constexpr int kDcStages = 2;
 constexpr uint32_t kDcA = 128 * 128;
 constexpr uint32_t kDcB = 256 * 128;
@@ -38,9 +40,9 @@ struct ConvArgs {
   int res_up2;          // residual is [B,Cout,H/2,W/2] and nearest-up-sampled on the fly (identity shortcut of an up block)
 };
 
-enum { DA_FULL = 0 /*4*/, DA_EMPTY = 4 /*4*/, DB_FULL = 8 /*2*/, DB_EMPTY = 10 /*2*/, DACC_FULL = 12, DACC_EMPTY = 13 };
+enum { DB_FULL = 0 /*2*/, DB_EMPTY = 2 /*2*/ };
 
-template <int kPasses>
+template <int kPasses, int N>
 __global__ void __launch_bounds__(kDcThreads, 1) conv_kernel(ConvArgs a) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -49,24 +51,16 @@ __global__ void __launch_bounds__(kDcThreads, 1) conv_kernel(ConvArgs a) {
   uint8_t* b_st = smem + 8 * kDcA;
   float* tab_bias = reinterpret_cast<float*>(b_st + kDcStages * kDcB);   // [512]
   uint64_t* bars = reinterpret_cast<uint64_t*>(tab_bias + 512);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 16);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // LeakyReLU in front of the convolution as max(v, slope * v), slope 1 = none: no run-time flag inside the unrolled loops
   const float lslope = a.pre_lrelu ? 0.2f : 1.f;
   for (int i = threadIdx.x; i < 512; i += blockDim.x) tab_bias[i] = (a.bias && i < a.Cout) ? a.bias[i] : 0.f;
   if (threadIdx.x == 0) {
-    for (int i = 0; i < 4; ++i) { mbar_init(bars + DA_FULL + i, 8); mbar_init(bars + DA_EMPTY + i, 1); }
-    for (int i = 0; i < kDcStages; ++i) { mbar_init(bars + DB_FULL + i, 1); mbar_init(bars + DB_EMPTY + i, 1); }
-    mbar_init(bars + DACC_FULL, 1);
-    mbar_init(bars + DACC_EMPTY, 8);
+    for (int i = 0; i < kDcStages; ++i) { mbar_init(bars + DB_FULL + i, 1); mbar_init(bars + DB_EMPTY + i, 2); }
     fence_mbar_init();
   }
-  if (warp == 8) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
   const int HW = a.H * a.W;
   const int Hs = a.up2 ? a.H >> 1 : a.H, Ws = a.up2 ? a.W >> 1 : a.W;
@@ -74,19 +68,25 @@ __global__ void __launch_bounds__(kDcThreads, 1) conv_kernel(ConvArgs a) {
   const int Cin = a.C1 + a.C2;
   const int taps = a.ksize * a.ksize;
   const int tiles_per_img = (HW + 127) / 128;
-  const int num_tiles = a.B * tiles_per_img;
-  const int my_tiles = (num_tiles - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);
+  const int num_items = a.B * tiles_per_img * a.nblocks;
+  const int my_items = (num_items - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);
   const int nchunks = a.kchunks;
   const int cblocks = a.small_cin ? 1 : Cin / 64;
   const uint32_t stage_bytes = static_cast<uint32_t>(a.Nb) * 128;
 
   if (warp < 8) {
     // ------------------------------------------------------------------ operand producer + epilogue
-    const int q = warp & 3, h = warp >> 2;
+    regs_inc<kMmaRegs>();
+    // warp (g, q, h): rows q*32.. (q = 2g or 2g+1, inside warpgroup g's 64) and channels h*32.. of every chunk
+    const int g = warp >> 2, q = 2 * g + (warp & 1), h = (warp >> 1) & 1, t = threadIdx.x & 127;
     const int row = q * 32 + lane;
+    const uint32_t a_off = g * 64 * 128;
     uint32_t cnt = 0;   // running chunk counter (ring position)
-    for (int it = 0; it < my_tiles; ++it) {
-      const int tile = blockIdx.x + it * gridDim.x;
+    uint32_t st = 0, ph = 0;
+    float d[N / 2];
+    for (int it = 0; it < my_items; ++it) {
+      const int item = blockIdx.x + it * gridDim.x;
+      const int tile = item / a.nblocks, nb = item % a.nblocks;
       const int b = tile / tiles_per_img, p0 = (tile % tiles_per_img) * 128;
       const int pix = p0 + row;
       const bool valid = pix < HW;
@@ -127,25 +127,42 @@ __global__ void __launch_bounds__(kDcThreads, 1) conv_kernel(ConvArgs a) {
           for (int j = 0; j < 32; ++j) asm volatile("ld.global.nc.f32 %0, [%1];" : "=f"(dst[j]) : "l"(src + j * HWs));
         }
       };
+      // one weight stage: wait, issue, and release the stage consumed one step earlier once its wgmmas are done
+      uint32_t prev = ~0u;
+      auto stage = [&](uint32_t a_tile, uint32_t a_tile2, bool two, bool accumulate) {
+        mbar_wait(bars + DB_FULL + st, ph);
+        acc_fence(d);
+        wgmma_fence();
+        const uint32_t bt = smem_u32(b_st + st * kDcB);
+        wg_k64<N>(d, a_tile, bt, accumulate);
+        if (two) wg_k64<N>(d, a_tile2, bt, true);
+        wgmma_commit();
+        wgmma_wait<1>();
+        acc_fence(d);
+        if (prev != ~0u && t == 0) mbar_arrive(bars + DB_EMPTY + prev);
+        prev = st;
+        if (++st == kDcStages) { st = 0; ph ^= 1; }
+      };
+      // a ring slot is rewritten four chunks later: by then every warp of the group has seen its wgmmas complete
       auto convert = [&](float (&cur)[32], bool in, int ck) {
         const uint32_t slot = cnt & 3;
-        mbar_wait(bars + DA_EMPTY + slot, ((cnt >> 2) & 1) ^ 1);
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
+        for (int gi = 0; gi < 4; ++gi) {
           float y[8];
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
-            float v = in ? cur[g * 8 + j] : 0.f;
+            float v = in ? cur[gi * 8 + j] : 0.f;
             v = fmaxf(v, lslope * v);
             y[j] = v;
           }
-          store_a8<kPasses == 3>(a_hi + slot * kDcA, a_lo + slot * kDcA, row, h * 32 + g * 8, y);
+          store_a8<kPasses == 3>(a_hi + slot * kDcA, a_lo + slot * kDcA, row, h * 32 + gi * 8, y);
         }
         fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bars + DA_FULL + slot);
+        named_barrier(1 + g, 128);
+        const uint32_t ahi = smem_u32(a_hi + slot * kDcA) + a_off, alo = smem_u32(a_lo + slot * kDcA) + a_off;
+        stage(ahi, alo, kPasses == 3, ck > 0);
+        if (kPasses == 3) stage(ahi, ahi, false, true);
         ++cnt;
-        (void)ck;
       };
       float xa[32], xb[32];
       bool ina = false, inb = false;
@@ -159,84 +176,37 @@ __global__ void __launch_bounds__(kDcThreads, 1) conv_kernel(ConvArgs a) {
         }
       }
 
-      // ---- epilogue
-      mbar_wait(bars + DACC_FULL, it & 1);
-      tc_fence_after();
-      for (int nb = 0; nb < a.nblocks; ++nb) {
-        for (int c0 = h * 32; c0 < a.Nb; c0 += 64) {
-          const int ch0 = nb * a.Nb + c0;
-          if (ch0 >= a.Cout) break;
-          uint32_t raw[32];
-          tmem_ld32(tmem + (static_cast<uint32_t>(q * 32) << 16) + nb * 256 + c0, raw);
-          const long obase = (static_cast<long>(b) * a.Cout + ch0) * HW + (valid ? pix : 0);
-          float res[32];
-          if (a.residual) {
-            const long rHW = a.res_up2 ? static_cast<long>(a.H >> 1) * (a.W >> 1) : HW;
-            const long rbase = (static_cast<long>(b) * a.Cout + ch0) * rHW +
-                               (a.res_up2 ? static_cast<long>(py >> 1) * (a.W >> 1) + (px >> 1) : (valid ? pix : 0));
+      // ---- epilogue straight from the fragments: rows 64g + frag_row, channels nb*Nb + frag_col
+      wgmma_wait<0>();
+      acc_fence(d);
+      if (t == 0) mbar_arrive(bars + DB_EMPTY + prev);
+      const long rHW = a.res_up2 ? static_cast<long>(a.H >> 1) * (a.W >> 1) : HW;
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const bool ok = ch0 + j < a.Cout;
-              float v;
-              asm volatile("ld.global.nc.f32 %0, [%1];" : "=f"(v) : "l"(a.residual + (ok ? rbase + static_cast<long>(j) * rHW : 0)));
-              res[j] = ok ? v : 0.f;
-            }
-          } else {
+      for (int i = 0; i < 2; ++i) {
+        const int epix = p0 + g * 64 + frag_row(t, i);
+        if (epix >= HW) continue;
+        const int ey = epix / a.W, ex = epix % a.W;
+        const long robase = a.res_up2 ? static_cast<long>(ey >> 1) * (a.W >> 1) + (ex >> 1) : epix;
 #pragma unroll
-            for (int j = 0; j < 32; ++j) res[j] = 0.f;
+        for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int c = frag_col(t, j, e), ch = nb * a.Nb + c;
+            if (c >= a.Nb || ch >= a.Cout) continue;
+            float v = d[4 * j + 2 * i + e] + tab_bias[ch];
+            if (a.residual) v += __ldg(a.residual + (static_cast<long>(b) * a.Cout + ch) * rHW + robase);
+            a.out[(static_cast<long>(b) * a.Cout + ch) * HW + epix] = v;
           }
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (valid && ch0 + j < a.Cout) a.out[obase + static_cast<long>(j) * HW] = __uint_as_float(raw[j]) + tab_bias[ch0 + j] + res[j];
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bars + DACC_EMPTY);
-    }
-  } else if (warp == 8) {
-    // ------------------------------------------------------------------ MMA issuer
-    {      // the warp walks the loops, one elected lane issues (umma.cuh: elect_one_sync)
-      const bool leader = elect_one_sync();
-      const uint32_t idesc = umma_idesc_bf16(128, a.Nb);
-      uint32_t st = 0, ph = 0, cnt = 0;
-      for (int it = 0; it < my_tiles; ++it) {
-        mbar_wait(bars + DACC_EMPTY, (it & 1) ^ 1);
-        tc_fence_after();
-        for (int ck = 0; ck < nchunks; ++ck, ++cnt) {
-          const uint32_t slot = cnt & 3;
-          mbar_wait(bars + DA_FULL + slot, (cnt >> 2) & 1);
-          tc_fence_after();
-          const uint32_t ahi = smem_u32(a_hi + slot * kDcA), alo = smem_u32(a_lo + slot * kDcA);
-          for (int nb = 0; nb < a.nblocks; ++nb) {
-            const uint32_t d = tmem + nb * 256;
-            mbar_wait(bars + DB_FULL + st, ph);
-            tc_fence_after();
-            umma_k64_if(leader, d, ahi, smem_u32(b_st + st * kDcB), idesc, ck > 0);
-            if (kPasses == 3) umma_k64_if(leader, d, alo, smem_u32(b_st + st * kDcB), idesc, true);
-            umma_commit_if(leader, bars + DB_EMPTY + st);
-            if (++st == kDcStages) { st = 0; ph ^= 1; }
-            if (kPasses == 3) {
-              mbar_wait(bars + DB_FULL + st, ph);
-              tc_fence_after();
-              umma_k64_if(leader, d, ahi, smem_u32(b_st + st * kDcB), idesc, true);
-              umma_commit_if(leader, bars + DB_EMPTY + st);
-              if (++st == kDcStages) { st = 0; ph ^= 1; }
-            }
-          }
-          umma_commit_if(leader, bars + DA_EMPTY + slot);
-        }
-        umma_commit_if(leader, bars + DACC_FULL);
       }
     }
   } else {
     // ------------------------------------------------------------------ weight producer
-    if (lane == 0) {
+    regs_dec<kProducerRegs>();
+    if (warp == 8 && lane == 0) {
       uint32_t st = 0, ph = 0;
-      for (int it = 0; it < my_tiles; ++it)
+      for (int it = 0; it < my_items; ++it) {
+        const int nb = (blockIdx.x + it * gridDim.x) % a.nblocks;
         for (int ck = 0; ck < nchunks; ++ck)
-          for (int nb = 0; nb < a.nblocks; ++nb)
             for (int part = 0; part < (kPasses == 3 ? 2 : 1); ++part) {
               mbar_wait_backoff(bars + DB_EMPTY + st, ph ^ 1);
               mbar_arrive_expect_tx(bars + DB_FULL + st, stage_bytes);
@@ -245,11 +215,17 @@ __global__ void __launch_bounds__(kDcThreads, 1) conv_kernel(ConvArgs a) {
                        bars + DB_FULL + st);
               if (++st == kDcStages) { st = 0; ph ^= 1; }
             }
+      }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 8) tmem_dealloc<512>(tmem);
+}
+
+template <int kPasses, int N>
+static int launch_conv(int grid, cudaStream_t st, const ConvArgs& a) {
+  const cudaError_t e = cudaFuncSetAttribute(conv_kernel<kPasses, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDcSmem);
+  if (e != cudaSuccess) { set_error("hg_conv2d: smem opt-in failed: %s", cudaGetErrorString(e)); return 2; }
+  conv_kernel<kPasses, N><<<grid, kDcThreads, kDcSmem, st>>>(a);
+  return check_launch("hg_conv2d");
 }
 
 // out[B,C,H,W] = P_a(a) + P_b(b) with P = 2x2 average pooling when the flag is set (source 2H x 2W),
@@ -337,7 +313,7 @@ int hg_conv2d(const float* x1, int C1, const float* x2, int C2, int B, int H, in
   const int Cin = C1 + C2, taps = ksize * ksize;
   // single-chunk contractions: the 3-channel stem and the 64 -> 1 / 26 heads.  A 64 -> 256 1x1 layer (the data gradient of an
   // up-sampling shortcut) also has taps * Cin == 64 but is an ordinary K = 64, N = 256 GEMM: tensor-core path (the SIMT kernel
-  // re-read x once per 32 output channels: 1.02 ms at B = 16, 256^2)
+  // re-read x once per 32 output channels)
   const int small = (taps * Cin <= 64 && !(Cin % 64 == 0 && Cout > 32)) ? 1 : 0;
   HG_REQUIRE(small || (C1 % 64 == 0 && C2 % 64 == 0), "hg_conv2d: channel counts must be multiples of 64 (or taps*Cin <= 64)");
   HG_REQUIRE(!small || C2 == 0, "hg_conv2d: the small-Cin path takes a single input");
@@ -355,20 +331,19 @@ int hg_conv2d(const float* x1, int C1, const float* x2, int C2, int B, int H, in
                                   passes, stream);
   hg::ConvArgs a{x1, x2, C1, C2, B, H, W, up2, pre_lrelu, ksize, static_cast<const uint8_t*>(wimg), Cout, Nb, nblocks,
                  small ? 1 : taps * Cin / 64, bias, residual, out, small, res_up2};
-  const int tiles = B * ((H * W + 127) / 128);
-  const int grid = tiles < hg::num_sms() ? tiles : hg::num_sms();
+  const int items = B * ((H * W + 127) / 128) * nblocks;
+  const int grid = items < hg::num_sms() ? items : hg::num_sms();
   auto st = static_cast<cudaStream_t>(stream);
-  cudaError_t e;
+  // wgmma N: the smallest of 64 / 128 / 256 that covers a block (columns past Nb are computed and dropped)
+  const int n = Nb <= 64 ? 64 : Nb <= 128 ? 128 : 256;
   if (passes == 3) {
-    e = cudaFuncSetAttribute(hg::conv_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, hg::kDcSmem);
-    if (e != cudaSuccess) { hg::set_error("hg_conv2d: smem opt-in failed: %s", cudaGetErrorString(e)); return 2; }
-    hg::conv_kernel<3><<<grid, hg::kDcThreads, hg::kDcSmem, st>>>(a);
-  } else {
-    e = cudaFuncSetAttribute(hg::conv_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, hg::kDcSmem);
-    if (e != cudaSuccess) { hg::set_error("hg_conv2d: smem opt-in failed: %s", cudaGetErrorString(e)); return 2; }
-    hg::conv_kernel<1><<<grid, hg::kDcThreads, hg::kDcSmem, st>>>(a);
+    if (n == 64) return hg::launch_conv<3, 64>(grid, st, a);
+    if (n == 128) return hg::launch_conv<3, 128>(grid, st, a);
+    return hg::launch_conv<3, 256>(grid, st, a);
   }
-  return hg::check_launch("hg_conv2d");
+  if (n == 64) return hg::launch_conv<1, 64>(grid, st, a);
+  if (n == 128) return hg::launch_conv<1, 128>(grid, st, a);
+  return hg::launch_conv<1, 256>(grid, st, a);
 }
 
 int hg_pool_add(const float* a, int pool_a, const float* b, int pool_b, float* out, long planes, int H, int W,

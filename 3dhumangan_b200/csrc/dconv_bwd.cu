@@ -1,17 +1,20 @@
 // Weight gradient of the discriminator's 3x3 / 1x1 convolutions (autograd through nn.Conv2d in
-// lib/discriminators/unet_discriminators.py:21-38), one launch per GROUP of filter taps and per 256-channel chunk
-// (as many taps as fit the 512 TMEM columns: ntaps * M-halves * ceil32(Cin chunk) <= 512, so dy is read once per group):
+// lib/discriminators/unet_discriminators.py:21-38), one launch per GROUP of filter taps and per output-channel chunk
+// (as many taps as fit the register accumulators: ntaps * M-halves * N <= 256 with N = the Cin chunk rounded up to 64, 128
+// or 256, so dy is read once per group):
 //     dW[co, ci, ky, kx] = sum_{b,h,w} dy[b, co, h, w] * x[b, ci, h + ky - pad, w + kx - pad]
 // Same machine as the SPADE weight gradient (csrc/synth_bwd.cu): K = pixels, both operands are K-major as stored
 // (NCHW planes are contiguous along W), the operand warps convert rows of 64 pixels into bf16 hi/lo SW128 images --
-// the x rows read through the tap's shift with zero padding at the image border -- and the [256 x Cin] fp32
-// accumulator stays in TMEM for the CTA's lifetime; per-CTA partials are reduced in fp64 in a fixed order.
+// the x rows read through the tap's shift with zero padding at the image border.  Warpgroup g issues the wgmmas of output
+// rows 64g..64g+63 of every M half; its fp32 accumulators stay in registers for the CTA's lifetime; per-CTA partials are
+// reduced in fp64 in a fixed order.
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hg {
 
-constexpr int kDwThreads = 288;
+constexpr int kDwThreads = 256;   // two warpgroups: operands, wgmma, drain
+constexpr int kDwCo = 128;        // output channels per work item of the whole-layer mode
 constexpr uint32_t kDwImg = 256 * 128;
 constexpr uint32_t kDwSmemBytes = 4 * kDwImg + 8 * 8 + 16 + 1024;
 
@@ -40,8 +43,8 @@ __device__ __forceinline__ ConvWgradItem conv_wgrad_item(int idx, int Cout, int 
   const int ngrp = (kk + per - 1) / per, nci_chunks = (Cin + 255) / 256;
   const int grp = idx % ngrp, cii = (idx / ngrp) % nci_chunks, coi = idx / (ngrp * nci_chunks);
   ConvWgradItem it;
-  it.co0 = coi * 256;
-  it.nco = Cout - it.co0 < 256 ? Cout - it.co0 : 256;
+  it.co0 = coi * kDwCo;
+  it.nco = Cout - it.co0 < kDwCo ? Cout - it.co0 : kDwCo;
   it.ci0 = cii * 256;
   it.nci = Cin - it.ci0 < 256 ? Cin - it.ci0 : 256;
   it.nq = (it.nci + 31) / 32 * 32;
@@ -50,32 +53,20 @@ __device__ __forceinline__ ConvWgradItem conv_wgrad_item(int idx, int Cout, int 
   return it;
 }
 
-enum { DW_AFULL = 0, DW_AEMPTY = 1, DW_BFULL = 2, DW_BEMPTY = 3, DW_DONE = 4 };
+// wgmma N for a chunk of nq input channels
+__host__ __device__ __forceinline__ int wgrad_n(int nq) { return nq <= 64 ? 64 : nq <= 128 ? 128 : 256; }
 
-template <int kPasses>
+// kN: wgmma N (>= nq); kNAcc = 256 / kN accumulators of [64 x kN] per warpgroup, one per (tap, M half)
+template <int kPasses, int kN>
 __global__ void __launch_bounds__(kDwThreads, 1) conv_wgrad_kernel(ConvWgradArgs a) {
+  constexpr int kNAcc = 256 / kN;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* s = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* a_hi = s;
   uint8_t* a_lo = s + kDwImg;
   uint8_t* b_hi = s + 2 * kDwImg;
   uint8_t* b_lo = s + 3 * kDwImg;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s + 4 * kDwImg);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    mbar_init(bars + DW_AFULL, 8);
-    mbar_init(bars + DW_AEMPTY, 1);
-    mbar_init(bars + DW_BFULL, 8);
-    mbar_init(bars + DW_BEMPTY, 1);
-    mbar_init(bars + DW_DONE, 1);
-    fence_mbar_init();
-  }
-  if (warp == 8) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
+  const int g = threadIdx.x >> 7, t128 = threadIdx.x & 127;
 
   if (a.layer) {
     const ConvWgradItem it = conv_wgrad_item(blockIdx.y, a.Cout, a.Cin, a.ksize, a.per);
@@ -94,12 +85,24 @@ __global__ void __launch_bounds__(kDwThreads, 1) conv_wgrad_kernel(ConvWgradArgs
   const int nmh = a.nco > 128 ? 2 : 1;          // M halves that carry rows
   const int nst_a = (a.nco + 31) >> 5, nst_b = a.nq >> 5;
 
-  if (warp < 8) {
+  float d[kNAcc][kN / 2];
+  // the operand images are single-buffered: both warpgroups' wgmmas that read them are complete before they are rewritten
+  auto images_free = [&]() {
+    wgmma_wait<0>();
+#pragma unroll
+    for (int ai = 0; ai < kNAcc; ++ai) acc_fence(d[ai]);
+    named_barrier(1, 256);
+  };
+  auto images_ready = [&]() {
+    fence_proxy_async_smem();
+    named_barrier(1, 256);
+  };
+  {
     const int sub = threadIdx.x & 7, rsub = threadIdx.x >> 3;
     float bsum[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) bsum[i] = 0.f;
-    uint32_t chunk = 0, bcnt = 0;
+    uint32_t chunk = 0;
     for (int it = 0; it < count; ++it) {
       const int tile = blockIdx.x + it * gridDim.x;
       const int b = tile / T, ti = tile - b * T;
@@ -129,7 +132,7 @@ __global__ void __launch_bounds__(kDwThreads, 1) conv_wgrad_kernel(ConvWgradArgs
             }
           }
         }
-        mbar_wait_sleep(bars + DW_AEMPTY, (chunk & 1) ^ 1);
+        images_free();
 #pragma unroll
         for (int st = 0; st < 8; ++st) {
           if (st >= nmh * 4) break;
@@ -138,9 +141,6 @@ __global__ void __launch_bounds__(kDwThreads, 1) conv_wgrad_kernel(ConvWgradArgs
           bsum[st] += ((y[0] + y[1]) + (y[2] + y[3])) + ((y[4] + y[5]) + (y[6] + y[7]));
           store_a8<kPasses == 3>(a_hi, a_lo, st * 32 + rsub, sub * 8, y);
         }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bars + DW_AFULL);
         // ---- x rows through each tap's shift (zero padding outside the image); re-reads hit L1/L2
         int ph[8], pw[8];
 #pragma unroll
@@ -150,7 +150,7 @@ __global__ void __launch_bounds__(kDwThreads, 1) conv_wgrad_kernel(ConvWgradArgs
           pw[j] = g - ph[j] * a.W;
         }
 #pragma unroll 1
-        for (int t = 0; t < a.ntaps; ++t, ++bcnt) {
+        for (int t = 0; t < a.ntaps; ++t) {
           const int oy = a.oy[t], ox = a.ox[t];
           bool ok[8];
 #pragma unroll
@@ -172,15 +172,28 @@ __global__ void __launch_bounds__(kDwThreads, 1) conv_wgrad_kernel(ConvWgradArgs
               for (int j = 0; j < 8; ++j) yq[st][j] = 0.f;
             }
           }
-          mbar_wait_sleep(bars + DW_BEMPTY, (bcnt & 1) ^ 1);
+          if (t > 0) images_free();
 #pragma unroll
           for (int st = 0; st < 8; ++st) {
             if (st >= nst_b) break;
             store_a8<kPasses == 3>(b_hi, b_lo, st * 32 + rsub, sub * 8, yq[st]);
           }
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bars + DW_BFULL);
+          images_ready();
+          // accumulator ai = t * nmh + mh: rows mh*128 + 64g.. of A against every row of B
+#pragma unroll
+          for (int ai = 0; ai < kNAcc; ++ai) {
+            if (ai / nmh != t) continue;
+            const int mh = ai % nmh;
+            const uint32_t ah = smem_u32(a_hi) + mh * (kDwImg / 2) + g * 64 * 128, al = ah + kDwImg;
+            acc_fence(d[ai]);
+            wgmma_fence();
+            wg_k64<kN>(d[ai], ah, smem_u32(b_hi), chunk > 0);
+            if (kPasses == 3) {
+              wg_k64<kN>(d[ai], al, smem_u32(b_hi), true);
+              wg_k64<kN>(d[ai], ah, smem_u32(b_lo), true);
+            }
+          }
+          wgmma_commit();
         }
       }
     }
@@ -192,67 +205,35 @@ __global__ void __launch_bounds__(kDwThreads, 1) conv_wgrad_kernel(ConvWgradArgs
       v += __shfl_xor_sync(0xffffffffu, v, 4);
       if (sub == 0) a.part_b[static_cast<long>(blockIdx.x) * 256 + st * 32 + rsub] = v;
     }
-  } else {      // MMA issuer: the warp walks the loops, one elected lane issues (umma.cuh: elect_one_sync)
-    const bool leader = elect_one_sync();
-    const uint32_t idesc = umma_idesc_bf16(128, a.nq);
-    uint32_t chunk = 0, bcnt = 0;
-    for (int it = 0; it < count; ++it)
-      for (int kc = 0; kc < 2; ++kc, ++chunk) {
-        mbar_wait_sleep(bars + DW_AFULL, chunk & 1);
-        for (int t = 0; t < a.ntaps; ++t, ++bcnt) {
-          mbar_wait_sleep(bars + DW_BFULL, bcnt & 1);
-          tc_fence_after();
-          for (int mh = 0; mh < nmh; ++mh) {
-            const uint32_t d = tmem + (t * nmh + mh) * a.nq;
-            const uint32_t ah = smem_u32(a_hi) + mh * (kDwImg / 2), al = smem_u32(a_lo) + mh * (kDwImg / 2);
-            umma_k64_if(leader, d, ah, smem_u32(b_hi), idesc, chunk > 0);
-            if (kPasses == 3) {
-              umma_k64_if(leader, d, al, smem_u32(b_hi), idesc, true);
-              umma_k64_if(leader, d, ah, smem_u32(b_lo), idesc, true);
-            }
-          }
-          umma_commit_if(leader, bars + DW_BEMPTY);
-        }
-        umma_commit_if(leader, bars + DW_AEMPTY);
-      }
-    umma_commit_if(leader, bars + DW_DONE);
   }
-  if (warp < 4) {
+  images_free();
+  // ---- drain: accumulator (tap t, M half mh) -> rows mh*128 + 64g + frag_row of the [256 x nq] partial of tap t
+  {
     float* dst0 = a.part_w + static_cast<long>(blockIdx.x) * a.ntaps * 256 * a.nq;
     if (count > 0) {
-      mbar_wait_long(bars + DW_DONE, 0);
-      tc_fence_after();
-      for (int t = 0; t < a.ntaps; ++t) {
+#pragma unroll
+      for (int ai = 0; ai < kNAcc; ++ai) {
+        if (ai >= a.ntaps * nmh) continue;
+        const int t = ai / nmh, mh = ai % nmh;
         float* dst = dst0 + static_cast<long>(t) * 256 * a.nq;
-        for (int mh = 0; mh < 2; ++mh) {
-          const int co = mh * 128 + warp * 32 + lane;
-          for (int cg = 0; cg < (a.nq >> 5); ++cg) {
-            uint32_t raw[32];
-            if (mh < nmh) {
-              tmem_ld32(tmem + (t * nmh + mh) * a.nq + (static_cast<uint32_t>(warp * 32) << 16) + cg * 32, raw);
-              tmem_ld_wait();
-            } else {
 #pragma unroll
-              for (int j = 0; j < 32; ++j) raw[j] = 0u;
-            }
-            float4* o = reinterpret_cast<float4*>(dst + static_cast<long>(co) * a.nq + cg * 32);
+        for (int i = 0; i < 2; ++i) {
+          const int co = mh * 128 + g * 64 + frag_row(t128, i);
 #pragma unroll
-            for (int j = 0; j < 8; ++j)
-              o[j] = make_float4(__uint_as_float(raw[4 * j]), __uint_as_float(raw[4 * j + 1]), __uint_as_float(raw[4 * j + 2]),
-                                 __uint_as_float(raw[4 * j + 3]));
+          for (int j = 0; j < kN / 8; ++j) {
+            const int c = frag_col(t128, j, 0);
+            if (c < a.nq) *reinterpret_cast<float2*>(dst + static_cast<long>(co) * a.nq + c) = make_float2(d[ai][4 * j + 2 * i], d[ai][4 * j + 2 * i + 1]);
           }
         }
       }
+      if (nmh == 1)     // rows 128..255 of every tap are zero
+        for (int t = 0; t < a.ntaps; ++t)
+          for (int i = threadIdx.x; i < 128 * a.nq; i += kDwThreads) dst0[static_cast<long>(t) * 256 * a.nq + 128 * a.nq + i] = 0.f;
     } else {
-      for (int i = threadIdx.x; i < a.ntaps * 256 * a.nq; i += 128) dst0[i] = 0.f;
+      for (int i = threadIdx.x; i < a.ntaps * 256 * a.nq; i += kDwThreads) dst0[i] = 0.f;
+      for (int i = threadIdx.x; i < 256; i += kDwThreads) a.part_b[static_cast<long>(blockIdx.x) * 256 + i] = 0.f;
     }
   }
-  if (count == 0 && warp >= 4 && warp < 8) {
-    for (int i = threadIdx.x - 128; i < 256; i += 128) a.part_b[static_cast<long>(blockIdx.x) * 256 + i] = 0.f;
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 8) tmem_dealloc<512>(tmem);
 }
 
 __global__ void conv_wgrad_reduce_kernel(const float* __restrict__ part_w, const float* __restrict__ part_b, int nparts,
@@ -295,6 +276,20 @@ __global__ void conv_wgrad_reduce_layer_kernel(const float* __restrict__ part_w,
   }
 }
 
+template <int kPasses, int kN>
+static cudaError_t launch_conv_wgrad_n(dim3 grid, cudaStream_t st, const ConvWgradArgs& a) {
+  const cudaError_t e = cudaFuncSetAttribute(conv_wgrad_kernel<kPasses, kN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kDwSmemBytes);
+  if (e == cudaSuccess) conv_wgrad_kernel<kPasses, kN><<<grid, kDwThreads, kDwSmemBytes, st>>>(a);
+  return e;
+}
+static cudaError_t launch_conv_wgrad(int passes, int n, dim3 grid, cudaStream_t st, const ConvWgradArgs& a) {
+  if (passes == 3)
+    return n == 64 ? launch_conv_wgrad_n<3, 64>(grid, st, a) : n == 128 ? launch_conv_wgrad_n<3, 128>(grid, st, a)
+                                                              : launch_conv_wgrad_n<3, 256>(grid, st, a);
+  return n == 64 ? launch_conv_wgrad_n<1, 64>(grid, st, a) : n == 128 ? launch_conv_wgrad_n<1, 128>(grid, st, a)
+                                                            : launch_conv_wgrad_n<1, 256>(grid, st, a);
+}
+
 }  // namespace hg
 
 extern "C" {
@@ -316,8 +311,9 @@ int hg_conv2d_wgrad_taps(const float* dy, const float* x, float* dw, float* dbia
              "hg_conv2d_wgrad_taps: dy / workspace must be 16-byte aligned");
   const int nq = (nci + 31) / 32 * 32;
   const int nmh = nco > 128 ? 2 : 1;
-  HG_REQUIRE(ntaps >= 1 && ntaps <= 9 && ntaps * nmh * nq <= 512,
-             "hg_conv2d_wgrad_taps: %d taps x %d M-halves x %d columns do not fit the 512 TMEM columns", ntaps, nmh, nq);
+  HG_REQUIRE(ntaps >= 1 && ntaps <= 9 && ntaps * nmh * hg::wgrad_n(nq) <= 256,
+             "hg_conv2d_wgrad_taps: %d taps x %d M-halves x %d columns do not fit the 256 accumulator columns", ntaps, nmh,
+             hg::wgrad_n(nq));
   hg::ConvWgradArgs a{};
   for (int t = 0; t < ntaps; ++t) {
     HG_REQUIRE(oy[t] >= -1 && oy[t] <= 1 && ox[t] >= -1 && ox[t] <= 1, "hg_conv2d_wgrad_taps: tap shift out of range");
@@ -333,14 +329,7 @@ int hg_conv2d_wgrad_taps(const float* dy, const float* x, float* dw, float* dbia
   a.B = B; a.H = H; a.W = W; a.Cout = Cout; a.Cin = Cin;
   a.co0 = co0; a.nco = nco; a.ci0 = ci0; a.nci = nci; a.nq = nq; a.ntaps = ntaps;
   auto st = static_cast<cudaStream_t>(stream);
-  cudaError_t e;
-  if (passes == 3) {
-    e = cudaFuncSetAttribute(hg::conv_wgrad_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, hg::kDwSmemBytes);
-    if (e == cudaSuccess) hg::conv_wgrad_kernel<3><<<grid, hg::kDwThreads, hg::kDwSmemBytes, st>>>(a);
-  } else {
-    e = cudaFuncSetAttribute(hg::conv_wgrad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, hg::kDwSmemBytes);
-    if (e == cudaSuccess) hg::conv_wgrad_kernel<1><<<grid, hg::kDwThreads, hg::kDwSmemBytes, st>>>(a);
-  }
+  const cudaError_t e = hg::launch_conv_wgrad(passes, hg::wgrad_n(nq), dim3(grid), st, a);
   if (e != cudaSuccess) { hg::set_error("hg_conv2d_wgrad_taps: smem opt-in failed: %s", cudaGetErrorString(e)); return 2; }
   int rc = hg::check_launch("hg_conv2d_wgrad_taps");
   if (rc) return rc;
@@ -354,12 +343,11 @@ int hg_conv2d_wgrad_taps(const float* dy, const float* x, float* dw, float* dbia
 // (16^2 .. 64^2 pixels: 2 .. 32 tiles per image) needed 9 .. 36 launches of 16-128 CTAs each with hg_conv2d_wgrad_taps.
 static void wgrad_layer_geometry(int B, int H, int W, int Cout, int Cin, int ksize, int* per, int* nitems, int* gx, long* item_stride) {
   const int kk = ksize * ksize;
-  const int nmh = Cout > 128 ? 2 : 1;
   const int nq_max = ((Cin < 256 ? Cin : 256) + 31) / 32 * 32;
-  *per = 512 / (nmh * nq_max) < 1 ? 1 : 512 / (nmh * nq_max);
+  *per = 256 / hg::wgrad_n(nq_max);        // one M half per item (kDwCo output channels)
   if (*per > kk) *per = kk;
   const int ngrp = (kk + *per - 1) / *per;
-  *nitems = ((Cout + 255) / 256) * ((Cin + 255) / 256) * ngrp;
+  *nitems = ((Cout + hg::kDwCo - 1) / hg::kDwCo) * ((Cin + 255) / 256) * ngrp;
   const int tiles = B * ((H * W + 127) / 128);
   // CTAs in flight: one per SM for a single item (every extra CTA is one more partial to drain and reduce), ~4 waves when the
   // grid is many small items of different cost
@@ -399,14 +387,8 @@ int hg_conv2d_wgrad_layer(const float* dy, const float* x, float* dW, float* dbi
   a.layer = 1; a.ksize = ksize; a.per = per; a.item_stride = stride;
   auto st = static_cast<cudaStream_t>(stream);
   const dim3 grid(gx, nitems);
-  cudaError_t e;
-  if (passes == 3) {
-    e = cudaFuncSetAttribute(hg::conv_wgrad_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, hg::kDwSmemBytes);
-    if (e == cudaSuccess) hg::conv_wgrad_kernel<3><<<grid, hg::kDwThreads, hg::kDwSmemBytes, st>>>(a);
-  } else {
-    e = cudaFuncSetAttribute(hg::conv_wgrad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, hg::kDwSmemBytes);
-    if (e == cudaSuccess) hg::conv_wgrad_kernel<1><<<grid, hg::kDwThreads, hg::kDwSmemBytes, st>>>(a);
-  }
+  const int nq_max = ((Cin < 256 ? Cin : 256) + 31) / 32 * 32;
+  const cudaError_t e = hg::launch_conv_wgrad(passes, hg::wgrad_n(nq_max), grid, st, a);
   if (e != cudaSuccess) { hg::set_error("hg_conv2d_wgrad_layer: smem opt-in failed: %s", cudaGetErrorString(e)); return 2; }
   int rc = hg::check_launch("hg_conv2d_wgrad_layer");
   if (rc) return rc;

@@ -2,35 +2,33 @@
 //
 // The first version (dconv.cu, still used for 1x1 / small maps / the 3-channel stem) builds nine shifted copies of every
 // [128 pixels x 64 channels] operand tile, one per filter tap: 9x the global loads and 9x the fp32 -> bf16 hi/lo
-// conversion work, which made the kernel producer-bound (22 % of the tensor pipe issued at B = 8, 512^2).
+// conversion work.
 //
-// Here a CTA owns a block of 2 image rows x 128 pixels (two M = 128 accumulator tiles).  For one chunk of 64 input channels it
-// converts the (2+2) x (128+2) haloed pixel block ONCE into the K-major SWIZZLE_128B operand layout (row = pixel, 520 rows)
-// and issues all nine taps by moving the START ADDRESS of the A descriptor: tap (dy, dx) of accumulator tile mt reads rows
-// ((mt + dy + 1) * 130 + dx + 1) ... + 127.  The swizzle of that layout is a function of the absolute shared-memory address
-// bits, so a descriptor that starts at any whole row (a multiple of 128 bytes, base_offset = 0) addresses the rows that were
-// written with the swizzle of their absolute row index -- verified on hardware by tools/experiments/desc_row_offset.cu.
-// Zero rows (outside the image) are the convolution's padding.  Both accumulator tiles share every weight stage, which also
-// halves the weight traffic from L2 per output pixel.
+// Here a CTA owns one image row of 128 output pixels (an M = 128 tile).  For one chunk of 64 input channels it converts the
+// 3 x (128+2) haloed pixel block ONCE into the K-major SWIZZLE_128B operand layout (row = pixel, 390 rows) and issues all
+// nine taps by moving the START ADDRESS of the A descriptor: tap (dy, dx) reads rows (dy + 1) * 130 + dx + 1 ... + 127.
+// The swizzle of that layout is a function of the absolute shared-memory address bits, so a descriptor that starts at any
+// whole row (a multiple of 128 bytes, base_offset = 0) addresses the rows that were written with the swizzle of their
+// absolute row index.  Zero rows (outside the image) are the convolution's padding.
 //
 // Folded in, exactly as in dconv.cu (unet_discriminators.py:20-54): LeakyReLU(0.2) and nearest 2x up-sampling in front of
 // the convolution, channel concatenation of two sources, bias, residual add (optionally of a half-resolution tensor).
 //
-// Warp roles (448 threads): 0-7 operand producers, 8-11 epilogue (TMEM -> NCHW planes), 12 MMA issuer, 13 weight producer.
-// TMEM: nsub <= 2 sub-blocks of <= 128 output channels x 2 pixel tiles; with nsub == 1 two accumulator sets alternate
-// between consecutive tiles so that the epilogue of tile t overlaps the MMAs of tile t+1.
+// Warp roles (384 threads): warpgroups 0-1 convert the operand block together, then warpgroup g issues the wgmmas of
+// pixels 64g..64g+63 (nsub <= 2 sub-blocks of <= 128 output channels, fp32 accumulators in registers) and stores them;
+// warp 8 streams the weight stages.
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hg {
 
-constexpr int kHcThreads = 448;
+constexpr int kHcThreads = 384;
 constexpr int kHcSeg = 130;                       // pixels per haloed row segment
-constexpr int kHcRows = 4 * kHcSeg;               // 520 operand rows
-constexpr uint32_t kHcA = 66 * 1024;              // 520 * 128 B rounded up to the 1024-byte swizzle pattern
+constexpr int kHcSegs = 3;                        // input rows y-1, y, y+1
+constexpr uint32_t kHcA = 50 * 1024;              // 390 * 128 B rounded up to the 1024-byte swizzle pattern
 constexpr int kHcBStages = 4;
 constexpr uint32_t kHcB = 128 * 128;              // [128 x 64] bf16
-constexpr uint32_t kHcSmem = 2 * kHcA + kHcBStages * kHcB + 256 * 4 + 32 * 8 + 16 + 1024;
+constexpr uint32_t kHcSmem = 2 * kHcA + kHcBStages * kHcB + 256 * 4 + 32 * 8 + 1024;
 static_assert(kHcSmem <= 232448, "shared memory budget");
 
 struct HaloArgs {
@@ -48,10 +46,10 @@ struct HaloArgs {
   float* out;
 };
 
-enum { HA_FULL = 0 /*4: one per row segment*/, HA_EMPTY = 4 /*4*/, HB_FULL = 8 /*4*/, HB_EMPTY = 12 /*4*/, HACC_FULL = 16 /*2*/,
-       HACC_EMPTY = 18 /*2*/ };
+enum { HB_FULL = 0 /*4*/, HB_EMPTY = 4 /*4*/ };
 
-template <int kPasses>
+// kN: wgmma N of one sub-block (>= nsubw)
+template <int kPasses, int kN>
 __global__ void __launch_bounds__(kHcThreads, 1) conv3x3_halo_kernel(HaloArgs a) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -60,54 +58,53 @@ __global__ void __launch_bounds__(kHcThreads, 1) conv3x3_halo_kernel(HaloArgs a)
   uint8_t* b_st = smem + 2 * kHcA;
   float* tab_bias = reinterpret_cast<float*>(b_st + kHcBStages * kHcB);   // [256]
   uint64_t* bars = reinterpret_cast<uint64_t*>(tab_bias + 256);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 32);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // LeakyReLU in front of the convolution as max(v, slope * v), slope 1 = none: no run-time flag inside the unrolled loops
   const float lslope = a.pre_lrelu ? 0.2f : 1.f;
   for (int i = threadIdx.x; i < 256; i += blockDim.x) tab_bias[i] = (a.bias && i < a.Cout) ? a.bias[i] : 0.f;
   if (threadIdx.x == 0) {
-    for (int i = 0; i < 4; ++i) { mbar_init(bars + HA_FULL + i, 8); mbar_init(bars + HA_EMPTY + i, 1); }
-    for (int i = 0; i < kHcBStages; ++i) { mbar_init(bars + HB_FULL + i, 1); mbar_init(bars + HB_EMPTY + i, 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(bars + HACC_FULL + i, 1); mbar_init(bars + HACC_EMPTY + i, 4); }
+    for (int i = 0; i < kHcBStages; ++i) { mbar_init(bars + HB_FULL + i, 1); mbar_init(bars + HB_EMPTY + i, 2); }
     fence_mbar_init();
   }
-  if (warp == 12) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
   const int HW = a.H * a.W;
   const int Hs = a.up2 ? a.H >> 1 : a.H, Ws = a.up2 ? a.W >> 1 : a.W;
   const long HWs = static_cast<long>(Hs) * Ws;
   const int Cin = a.C1 + a.C2;
   const int cblocks = Cin / 64;
-  const int xtiles = a.W / 128, ytiles = a.H / 2;
-  const int num_tiles = a.B * ytiles * xtiles;
+  const int xtiles = a.W / 128;
+  const int num_tiles = a.B * a.H * xtiles;
   const int my_tiles = (num_tiles - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);
-  const int nsets = a.nsub == 1 ? 2 : 1;
   const uint32_t stage_bytes = static_cast<uint32_t>(a.nsubw) * 128;
 
   if (warp < 8) {
-    // ------------------------------------------------------------------ operand producers
-    // The operand buffer of a chunk is FOUR row segments with their own full / empty barriers: the MMA thread walks the taps
-    // dy = -1, 0, +1 (segments {0,1}, {1,2}, {2,3} for the two pixel tiles), so segment 0 of the NEXT chunk can be rebuilt
-    // after a third of this chunk's MMAs, segment 1 after two thirds -- the producers (latency-bound on their loads) overlap
-    // the MMAs although the buffer is not duplicated.
+    regs_inc<kMmaRegs>();
     const int t = threadIdx.x;                 // 0..255
+    const int g = t >> 7, t128 = t & 127;
     const int px = t & 127, half = t >> 7;     // one interior pixel, 32 of the chunk's 64 channels (two batches of 16)
     const int hside = t >> 3, hg8 = t & 7;     // threads 0..15: halo pixel (left / right), 8 channels
-    uint32_t n = 0;                            // chunk counter (segment barrier phase)
+    float d[2][kN / 2];
+    uint32_t st = 0, ph = 0, prev = ~0u;
+    // the operand block is single-buffered: both warpgroups' wgmmas of the previous chunk are complete before it is rebuilt
+    auto operands_free = [&]() {
+      wgmma_wait<0>();
+      acc_fence(d[0]);
+      acc_fence(d[1]);
+      if (prev != ~0u && t128 == 0) mbar_arrive(bars + HB_EMPTY + prev);
+      prev = ~0u;
+      named_barrier(1, 256);
+    };
     for (int it = 0; it < my_tiles; ++it) {
       const int tile = blockIdx.x + it * gridDim.x;
-      const int xb = tile % xtiles, yb = (tile / xtiles) % ytiles, b = tile / (xtiles * ytiles);
-      const int x0 = xb * 128, y0 = yb * 2;
+      const int xb = tile % xtiles, y0 = (tile / xtiles) % a.H, b = tile / (xtiles * a.H);
+      const int x0 = xb * 128;
       const int sx = a.up2 ? (x0 + px) >> 1 : x0 + px;
       const int hx = hside ? x0 + 128 : x0 - 1;
       const bool hxok = t < 16 && hx >= 0 && hx < a.W;
       const int hsx = hxok ? (a.up2 ? hx >> 1 : hx) : 0;
-      for (int cb = 0; cb < cblocks; ++cb, ++n) {
+      for (int cb = 0; cb < cblocks; ++cb) {
         const int c0 = cb * 64;
         const float* plane = c0 < a.C1 ? a.x1 + (static_cast<long>(b) * a.C1 + c0) * HWs
                                        : a.x2 + (static_cast<long>(b) * a.C2 + (c0 - a.C1)) * HWs;
@@ -134,21 +131,21 @@ __global__ void __launch_bounds__(kHcThreads, 1) conv3x3_halo_kernel(HaloArgs a)
           rowinfo(bi >> 1, ok, off);
           const uint32_t row = (bi >> 1) * kHcSeg + 1 + px;
 #pragma unroll
-          for (int g = 0; g < 2; ++g) {
+          for (int gi = 0; gi < 2; ++gi) {
             float y[8];
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
-              float val = ok ? cur[g * 8 + j] : 0.f;
+              float val = ok ? cur[gi * 8 + j] : 0.f;
               val = fmaxf(val, lslope * val);
               y[j] = val;
             }
-            store_a8<kPasses == 3>(a_hi, a_lo, row, half * 32 + (bi & 1) * 16 + g * 8, y);
+            store_a8<kPasses == 3>(a_hi, a_lo, row, half * 32 + (bi & 1) * 16 + gi * 8, y);
           }
         };
         issue(v[0], 0);
         issue(v[1], 1);
 #pragma unroll
-        for (int s = 0; s < 4; ++s) {
+        for (int s = 0; s < kHcSegs; ++s) {
           // halo pixels of this segment (threads 0..15), loaded before the wait like the batches above
           float hv[8];
           bool hok = false;
@@ -164,11 +161,11 @@ __global__ void __launch_bounds__(kHcThreads, 1) conv3x3_halo_kernel(HaloArgs a)
               src += HWs;
             }
           }
-          mbar_wait(bars + HA_EMPTY + s, (n & 1) ^ 1);
+          if (s == 0) operands_free();
           convert(v[0], 2 * s);
-          if (s < 3) issue(v[0], 2 * s + 2);
+          if (s < kHcSegs - 1) issue(v[0], 2 * s + 2);
           convert(v[1], 2 * s + 1);
-          if (s < 3) issue(v[1], 2 * s + 3);
+          if (s < kHcSegs - 1) issue(v[1], 2 * s + 3);
           if (t < 16) {
             float y[8];
 #pragma unroll
@@ -179,130 +176,68 @@ __global__ void __launch_bounds__(kHcThreads, 1) conv3x3_halo_kernel(HaloArgs a)
             }
             store_a8<kPasses == 3>(a_hi, a_lo, s * kHcSeg + (hside ? kHcSeg - 1 : 0), hg8 * 8, y);
           }
-          fence_proxy_async_smem();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bars + HA_FULL + s);
         }
-      }
-    }
-  } else if (warp < 12) {
-    // ------------------------------------------------------------------ epilogue
-    const int q = warp - 8;
-    for (int it = 0; it < my_tiles; ++it) {
-      const int tile = blockIdx.x + it * gridDim.x;
-      const int xb = tile % xtiles, yb = (tile / xtiles) % ytiles, b = tile / (xtiles * ytiles);
-      const int x = xb * 128 + q * 32 + lane;
-      const int set = it % nsets;
-      mbar_wait_sleep(bars + HACC_FULL + set, (it / nsets) & 1);
-      tc_fence_after();
-      for (int mt = 0; mt < 2; ++mt) {
-        const int y = yb * 2 + mt;
-        const long pix = static_cast<long>(y) * a.W + x;
-        for (int sb = 0; sb < a.nsub; ++sb) {
-          for (int c0 = 0; c0 < a.nsubw; c0 += 16) {
-            const int ch0 = sb * a.nsubw + c0;
-            if (ch0 >= a.Cout) break;
-            uint32_t raw[16];
-            tmem_ld16(tmem + (static_cast<uint32_t>(q * 32) << 16) + set * 256 + (mt * a.nsub + sb) * 128 + c0, raw);
-            float res[16];
-            if (a.residual) {
-              const long rHW = a.res_up2 ? static_cast<long>(a.H >> 1) * (a.W >> 1) : HW;
-              const float* rp = a.residual + (static_cast<long>(b) * a.Cout + ch0) * rHW +
-                                (a.res_up2 ? static_cast<long>(y >> 1) * (a.W >> 1) + (x >> 1) : pix);
+        fence_proxy_async_smem();
+        named_barrier(1, 256);
+        // ---- nine taps x nsub sub-blocks: warpgroup g reads pixel rows 64g.. of each tap's shifted window
+        const uint32_t ahi = smem_u32(a_hi) + g * 64 * 128, alo = smem_u32(a_lo) + g * 64 * 128;
+        for (int tap = 0; tap < 9; ++tap) {
+          const int dy = tap / 3 - 1, dx = tap % 3 - 1;
+          const uint32_t r0 = static_cast<uint32_t>((dy + 1) * kHcSeg + dx + 1) * 128u;
+          const bool first = cb == 0 && tap == 0;
 #pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                const bool ok = ch0 + j < a.Cout;
-                float v;
-                asm volatile("ld.global.nc.f32 %0, [%1];" : "=f"(v) : "l"(ok ? rp : a.residual));
-                res[j] = ok ? v : 0.f;
-                rp += rHW;
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 16; ++j) res[j] = 0.f;
-            }
-            tmem_ld_wait();
-            float* op = a.out + (static_cast<long>(b) * a.Cout + ch0) * HW + pix;
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              if (ch0 + j < a.Cout) *op = __uint_as_float(raw[j]) + tab_bias[ch0 + j] + res[j];
-              op += HW;
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bars + HACC_EMPTY + set);
-    }
-  } else if (warp == 12) {
-    // ------------------------------------------------------------------ MMA issuer
-    // The whole warp walks the loops and polls the barriers; one elected lane issues.  With the loops inside `if (lane == 0)`
-    // every loop variable lived in vector registers of a divergent region and each tcgen05.mma cost 17.5 instructions
-    // (5 R2UR, 3 PLOP3, ELECT, ...; ncu: the issuing warp busy 80 % of the time, ~135 cycles per MMA whose tensor work is
-    // 64 (N = 128) or 32 (N = 64) cycles); in convergent code descriptors and addresses stay in uniform registers.
-    {
-      const bool leader = elect_one_sync();
-      const uint32_t idesc = umma_idesc_bf16(128, a.nsubw);
-      const uint32_t ahi = smem_u32(a_hi), alo = smem_u32(a_lo);
-      uint32_t st = 0, ph = 0, n = 0;
-      for (int it = 0; it < my_tiles; ++it) {
-        const int set = it % nsets;
-        mbar_wait(bars + HACC_EMPTY + set, ((it / nsets) & 1) ^ 1);
-        tc_fence_after();
-        for (int cb = 0; cb < cblocks; ++cb, ++n) {
-          for (int tap = 0; tap < 9; ++tap) {
-            const int dy = tap / 3 - 1, dx = tap % 3 - 1;
-            if (dx == -1) {       // first tap of a filter row: its two segments are {dy + 1, dy + 2}
-              if (dy == -1) mbar_wait(bars + HA_FULL + 0, n & 1);
-              mbar_wait(bars + HA_FULL + dy + 2, n & 1);
-              tc_fence_after();
-            }
-            const uint32_t r0 = static_cast<uint32_t>((dy + 1) * kHcSeg + dx + 1) * 128u;    // pixel tile mt = 0
-            const uint32_t r1 = r0 + kHcSeg * 128u;                                          // pixel tile mt = 1
-            const bool first = cb == 0 && tap == 0;
-            for (int sb = 0; sb < a.nsub; ++sb) {
-              const uint32_t d0 = tmem + set * 256 + sb * 128, d1 = d0 + a.nsub * 128;
+          for (int sb = 0; sb < 2; ++sb) {
+            if (sb >= a.nsub) continue;
+            // one weight stage: wait, issue, and release the stage consumed one step earlier once its wgmmas are done
+            auto stage = [&](uint32_t a_tile, uint32_t a_tile2, bool two, bool accumulate) {
               mbar_wait(bars + HB_FULL + st, ph);
-              tc_fence_after();
-              uint32_t bt = smem_u32(b_st + st * kHcB);
-              if (leader) {
-                umma_k64(d0, ahi + r0, bt, idesc, !first);
-                umma_k64(d1, ahi + r1, bt, idesc, !first);
-                if (kPasses == 3) {
-                  umma_k64(d0, alo + r0, bt, idesc, true);
-                  umma_k64(d1, alo + r1, bt, idesc, true);
-                }
-                umma_commit(bars + HB_EMPTY + st);
-              }
-              __syncwarp();
+              acc_fence(d[sb]);
+              wgmma_fence();
+              const uint32_t bt = smem_u32(b_st + st * kHcB);
+              wg_k64<kN>(d[sb], a_tile, bt, accumulate);
+              if (two) wg_k64<kN>(d[sb], a_tile2, bt, true);
+              wgmma_commit();
+              wgmma_wait<1>();
+              acc_fence(d[0]);
+              acc_fence(d[1]);
+              if (prev != ~0u && t128 == 0) mbar_arrive(bars + HB_EMPTY + prev);
+              prev = st;
               if (++st == kHcBStages) { st = 0; ph ^= 1; }
-              if (kPasses == 3) {
-                mbar_wait(bars + HB_FULL + st, ph);
-                tc_fence_after();
-                bt = smem_u32(b_st + st * kHcB);
-                if (leader) {
-                  umma_k64(d0, ahi + r0, bt, idesc, true);
-                  umma_k64(d1, ahi + r1, bt, idesc, true);
-                  umma_commit(bars + HB_EMPTY + st);
-                }
-                __syncwarp();
-                if (++st == kHcBStages) { st = 0; ph ^= 1; }
-              }
-            }
-            if (dx == 1 && leader) {   // last tap of a filter row: segment dy + 1 is not read again (dy = +1: nor is segment 3)
-              umma_commit(bars + HA_EMPTY + dy + 1);
-              if (dy == 1) umma_commit(bars + HA_EMPTY + 3);
-            }
+            };
+            stage(ahi + r0, alo + r0, kPasses == 3, !first);
+            if (kPasses == 3) stage(ahi + r0, ahi + r0, false, true);
           }
         }
-        if (leader) umma_commit(bars + HACC_FULL + set);
-        __syncwarp();
+      }
+      operands_free();
+      // ---- epilogue straight from the fragments: pixel x0 + 64g + frag_row, channel sb * nsubw + frag_col
+      const long pixrow = static_cast<long>(y0) * a.W;
+#pragma unroll
+      for (int sb = 0; sb < 2; ++sb) {
+        if (sb >= a.nsub) continue;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int x = x0 + g * 64 + frag_row(t128, i);
+          const long pix = pixrow + x;
+          const long rpix = a.res_up2 ? static_cast<long>(y0 >> 1) * (a.W >> 1) + (x >> 1) : pix;
+          const long rHW = a.res_up2 ? static_cast<long>(a.H >> 1) * (a.W >> 1) : HW;
+#pragma unroll
+          for (int j = 0; j < kN / 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int c = frag_col(t128, j, e), ch = sb * a.nsubw + c;
+              if (c >= a.nsubw || ch >= a.Cout) continue;
+              float val = d[sb][4 * j + 2 * i + e] + tab_bias[ch];
+              if (a.residual) val += __ldg(a.residual + (static_cast<long>(b) * a.Cout + ch) * rHW + rpix);
+              a.out[(static_cast<long>(b) * a.Cout + ch) * HW + pix] = val;
+            }
+        }
       }
     }
   } else {
     // ------------------------------------------------------------------ weight producer
-    if (lane == 0) {
+    regs_dec<kProducerRegs>();
+    if (warp == 8 && lane == 0) {
       uint32_t st = 0, ph = 0;
       const size_t tile_bytes = static_cast<size_t>(a.Nb) * 128;       // one packed [Nb x 64] part
       for (int it = 0; it < my_tiles; ++it)
@@ -324,9 +259,14 @@ __global__ void __launch_bounds__(kHcThreads, 1) conv3x3_halo_kernel(HaloArgs a)
           }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 12) tmem_dealloc<512>(tmem);
+}
+
+template <int kPasses, int kN>
+static int launch_halo(int grid, cudaStream_t st, const HaloArgs& a) {
+  const cudaError_t e = cudaFuncSetAttribute(conv3x3_halo_kernel<kPasses, kN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kHcSmem);
+  if (e != cudaSuccess) { set_error("hg_conv2d (halo): smem opt-in failed: %s", cudaGetErrorString(e)); return 2; }
+  conv3x3_halo_kernel<kPasses, kN><<<grid, kHcThreads, kHcSmem, st>>>(a);
+  return check_launch("hg_conv2d (halo)");
 }
 
 }  // namespace hg
@@ -341,25 +281,16 @@ int hg_conv3x3_halo_launch(const float* x1, int C1, const float* x2, int C2, int
   const int nsub = (Cout + nsubw - 1) / nsubw;
   hg::HaloArgs a{x1, x2, C1, C2, B, H, W, up2, pre_lrelu, static_cast<const uint8_t*>(wimg), Cout, Nb, 9 * Cin / 64,
                  nsub, nsubw, bias, residual, res_up2, out};
-  const int tiles = B * (H / 2) * (W / 128);
+  const int tiles = B * H * (W / 128);
   const int grid = tiles < hg::num_sms() ? tiles : hg::num_sms();
   auto st = static_cast<cudaStream_t>(stream);
-  cudaError_t e;
-  if (passes == 3) {
-    e = cudaFuncSetAttribute(hg::conv3x3_halo_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, hg::kHcSmem);
-    if (e != cudaSuccess) { hg::set_error("hg_conv2d (halo): smem opt-in failed: %s", cudaGetErrorString(e)); return 2; }
-    hg::conv3x3_halo_kernel<3><<<grid, hg::kHcThreads, hg::kHcSmem, st>>>(a);
-  } else {
-    e = cudaFuncSetAttribute(hg::conv3x3_halo_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, hg::kHcSmem);
-    if (e != cudaSuccess) { hg::set_error("hg_conv2d (halo): smem opt-in failed: %s", cudaGetErrorString(e)); return 2; }
-    hg::conv3x3_halo_kernel<1><<<grid, hg::kHcThreads, hg::kHcSmem, st>>>(a);
-  }
-  return hg::check_launch("hg_conv2d (halo)");
+  if (passes == 3) return nsubw <= 64 ? hg::launch_halo<3, 64>(grid, st, a) : hg::launch_halo<3, 128>(grid, st, a);
+  return nsubw <= 64 ? hg::launch_halo<1, 64>(grid, st, a) : hg::launch_halo<1, 128>(grid, st, a);
 }
 
 // shapes the haloed kernel covers (everything else stays on dconv.cu's kernel)
 bool hg_conv3x3_halo_eligible(int C1, int C2, int H, int W, int ksize, int Cout, int Nb) {
-  if (ksize != 3 || W % 128 != 0 || H % 2 != 0) return false;
+  if (ksize != 3 || W % 128 != 0) return false;
   if (C1 % 64 != 0 || C2 % 64 != 0) return false;
   if (Cout > 256) return false;
   const int nsubw = Nb > 128 ? 128 : Nb;

@@ -3,11 +3,10 @@
 // tiles would be almost empty (K = 27 of 64) and the layers are bound by the 0.5-1 GB they write / read, so they run as a plain
 // fp32 SIMT kernel: a thread owns one output pixel and 32 output channels, the K <= 64 inputs of its patch live in registers,
 // the weights of the channel group in shared memory (fp32 rebuilt from the packed bf16 hi + lo image: 2^-17 relative, products
-// and sums in fp32) are read as broadcast float4.  The first tensor-core kernel spent ~1 ms on each of these layers at B = 8,
-// 512^2 (0.17 ms of HBM time); same fused options (LeakyReLU / nearest 2x up-sampling in front, bias, residual).
+// and sums in fp32) are read as broadcast float4.  Same fused options (LeakyReLU / nearest 2x up-sampling in front, bias, residual).
 #include <cuda_bf16.h>
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hg {
 

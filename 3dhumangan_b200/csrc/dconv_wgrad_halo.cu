@@ -3,24 +3,26 @@
 // GEMM view per filter tap: D_tap[co, ci] += A[co, K = pixels] . B_tap[ci, K = pixels]^T.
 //
 // The first version (dconv_bwd.cu) rebuilds the B operand (rows = input channels, K-major along the pixels) once PER TAP from
-// global memory through the tap's shift: nine times the loads and conversions, B single-buffered -- 13-15 % of HBM, 12-14 %
-// tensor-active, 2134 launches per training iteration.
+// global memory through the tap's shift: nine times the loads and conversions, B single-buffered, and many launches per
+// training iteration.
 //
 // Here the input is converted ONCE per image-row segment into the operand image the forward kernel uses (dconv_halo.cu):
-// row = pixel (x0-1 .. x0+128), 128-byte row = 64 channels, SWIZZLE_128B.  Read as an MN-MAJOR B operand (instruction
-// descriptor bit 16) that image has K = pixel rows and N = channels contiguous, so a filter tap is again nothing but a ROW
-// offset of the descriptor start ((dy) selects the ring slot of image row y + dy, (dx) moves the start by one row) -- both
-// properties verified on hardware by tools/experiments/desc_mn_major.cu.  A = dy rows are K-major as stored in NCHW.
-// A CTA walks down strips of image rows with a 4-slot ring of input rows (each input row is converted once and used by the
-// three output rows around it) and double-buffered 64-pixel chunks of dy; the [ntaps x 128 x 64] fp32 accumulators live in
-// TMEM for the CTA's lifetime (ntaps * 64 <= 512 columns => at most 8 taps per launch: a 3x3 filter takes two launches per
-// (128 output, 64 input)-channel block); per-CTA partials are reduced in fp64 in a fixed order (deterministic).
+// row = pixel (x0-1 .. x0+128), 128-byte row = 64 channels, SWIZZLE_128B.  Read as an MN-MAJOR B operand (wgmma with B
+// transposed) that image has K = pixel rows and N = channels contiguous, so a filter tap is again nothing but a ROW offset of
+// the descriptor start ((dy) selects the ring slot of image row y + dy, (dx) moves the start by one row).  A = dy rows are
+// K-major as stored in NCHW.  A CTA walks down strips of image rows with a 4-slot ring of input rows (each input row is
+// converted once and used by the three output rows around it) and double-buffered 64-pixel chunks of dy.  Two warpgroups
+// build the operands together; warpgroup g issues the wgmmas of output channels 64g..64g+63 and keeps their
+// [ntaps x 64 x 64] fp32 accumulators in registers for the CTA's lifetime (at most 4 taps per launch: a 3x3 filter takes
+// three launches, one per filter row, per (128 output, 64 input)-channel block); per-CTA partials are reduced in fp64 in a
+// fixed order (deterministic).
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hg {
 
-constexpr int kWhThreads = 416;                   // warps 0-7 producers, 8-11 epilogue, 12 MMA issuer
+constexpr int kWhThreads = 256;                   // two warpgroups: operands, wgmma, drain
+constexpr int kWhMaxTaps = 4;
 constexpr int kWhSeg = 130;
 constexpr uint32_t kWhX = 66 * 1024;              // 4 slots x 130 rows x 128 B, rounded to the swizzle pattern
 constexpr uint32_t kWhDy = 128 * 128;             // [128 co x 64 px] bf16
@@ -35,12 +37,10 @@ struct WgHaloArgs {
   int B, H, W, Cout, Cin;
   int co0, nco;          // <= 128 rows of dy
   int ci0, nci;          // <= 64 rows of x
-  int ntaps;             // <= 8
-  int tdy[8], tdx[8];    // tap t reads x at (y + tdy, x + tdx)
+  int ntaps;             // <= kWhMaxTaps
+  int tdy[kWhMaxTaps], tdx[kWhMaxTaps];    // tap t reads x at (y + tdy, x + tdx)
   int strip;             // image rows per work unit
 };
-
-enum { WX_FULL = 0 /*4*/, WX_EMPTY = 4 /*4*/, WD_FULL = 8 /*2*/, WD_EMPTY = 10 /*2*/, WH_DONE = 12 };
 
 template <int kPasses>
 __global__ void __launch_bounds__(kWhThreads, 1) conv3x3_wgrad_halo_kernel(WgHaloArgs a) {
@@ -50,20 +50,7 @@ __global__ void __launch_bounds__(kWhThreads, 1) conv3x3_wgrad_halo_kernel(WgHal
   uint8_t* x_lo = smem + kWhX;
   uint8_t* d_hi = smem + 2 * kWhX;               // 2 chunk buffers
   uint8_t* d_lo = d_hi + 2 * kWhDy;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(d_lo + 2 * kWhDy);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 32);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < 4; ++i) { mbar_init(bars + WX_FULL + i, 8); mbar_init(bars + WX_EMPTY + i, 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(bars + WD_FULL + i, 8); mbar_init(bars + WD_EMPTY + i, 1); }
-    mbar_init(bars + WH_DONE, 1);
-    fence_mbar_init();
-  }
-  if (warp == 12) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
+  const int g = threadIdx.x >> 7, t128 = threadIdx.x & 127;
 
   const int HW = a.H * a.W;
   const int xtiles = a.W / 128, ystrips = a.H / a.strip;
@@ -71,13 +58,27 @@ __global__ void __launch_bounds__(kWhThreads, 1) conv3x3_wgrad_halo_kernel(WgHal
   const int my_units = (units - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);
   const int S = a.strip;
 
-  if (warp < 8) {
-    // ------------------------------------------------------------------ producers
+  float d[kWhMaxTaps][32];
+  // Operands are rewritten only after both warpgroups' wgmmas have completed (the ring slot / dy buffer that is refilled was
+  // read two output rows / two chunks earlier; waiting for all of them keeps the protocol to two barriers per fill).
+  auto operands_free = [&]() {
+    wgmma_wait<0>();
+#pragma unroll
+    for (int tp = 0; tp < kWhMaxTaps; ++tp) acc_fence(d[tp]);
+    named_barrier(1, 256);
+  };
+  auto operands_ready = [&]() {
+    fence_proxy_async_smem();
+    named_barrier(1, 256);
+  };
+  {
+    // ------------------------------------------------------------------ producers + wgmma
     const int t = threadIdx.x;
     const int px = t & 127, half = t >> 7;       // x rows: one pixel, 32 channels
     const int sub = t & 7, rsub = t >> 3;        // dy: 8-pixel group, output-channel row (+ 32 i)
     float bsum[4] = {0.f, 0.f, 0.f, 0.f};
-    uint32_t xcnt = 0, dcnt = 0;
+    uint32_t xcnt = 0, dcnt = 0, xbase = 0;
+    bool started = false;
     for (int u = 0; u < my_units; ++u) {
       const int unit = blockIdx.x + u * gridDim.x;
       const int xb = unit % xtiles, ys = (unit / xtiles) % ystrips, b = unit / (xtiles * ystrips);
@@ -116,7 +117,7 @@ __global__ void __launch_bounds__(kWhThreads, 1) conv3x3_wgrad_halo_kernel(WgHal
             src += HW;
           }
         }
-        mbar_wait_sleep(bars + WX_EMPTY + slot, ((xcnt >> 2) & 1) ^ 1);
+        operands_free();
         const uint32_t row = slot * kWhSeg + 1 + px;
 #pragma unroll
         for (int q = 0; q < 2; ++q) {
@@ -129,9 +130,7 @@ __global__ void __launch_bounds__(kWhThreads, 1) conv3x3_wgrad_halo_kernel(WgHal
           }
         }
         if (t < 16) store_a8<kPasses == 3>(x_hi, x_lo, slot * kWhSeg + (hside ? kWhSeg - 1 : 0), hg8 * 8, hv);
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bars + WX_FULL + slot);
+        operands_ready();
         ++xcnt;
       };
       auto fill_dy = [&](int y, int c) {         // 64 pixels x0 + 64 c .. of image row y -> chunk buffer dcnt & 1
@@ -149,7 +148,7 @@ __global__ void __launch_bounds__(kWhThreads, 1) conv3x3_wgrad_halo_kernel(WgHal
             va[2 * i] = va[2 * i + 1] = make_float4(0.f, 0.f, 0.f, 0.f);
           }
         }
-        mbar_wait_sleep(bars + WD_EMPTY + buf, ((dcnt >> 1) & 1) ^ 1);
+        operands_free();
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
           const float yv[8] = {va[2 * i].x, va[2 * i].y, va[2 * i].z, va[2 * i].w,
@@ -157,10 +156,34 @@ __global__ void __launch_bounds__(kWhThreads, 1) conv3x3_wgrad_halo_kernel(WgHal
           bsum[i] += ((yv[0] + yv[1]) + (yv[2] + yv[3])) + ((yv[4] + yv[5]) + (yv[6] + yv[7]));
           store_a8<kPasses == 3>(d_hi + buf * kWhDy, d_lo + buf * kWhDy, rsub + 32 * i, sub * 8, yv);
         }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bars + WD_FULL + buf);
+        operands_ready();
         ++dcnt;
+      };
+      // output row i, pixel chunk c: every tap of this launch on dy chunk buffer (dcnt - 1) & 1
+      auto mma = [&](int i, int c) {
+        const uint32_t buf = (dcnt - 1) & 1;
+        const uint32_t ah = smem_u32(d_hi + buf * kWhDy) + g * 64 * 128, al = smem_u32(d_lo + buf * kWhDy) + g * 64 * 128;
+        const uint32_t xh = smem_u32(x_hi), xl = smem_u32(x_lo);
+#pragma unroll
+        for (int tp = 0; tp < kWhMaxTaps; ++tp) {
+          if (tp >= a.ntaps) continue;
+          const uint32_t slot = (xbase + i + 1 + a.tdy[tp]) & 3;
+          const uint32_t brow = (slot * kWhSeg + 1 + a.tdx[tp] + c * 64) * 128u;
+          acc_fence(d[tp]);
+          wgmma_fence();
+#pragma unroll
+          for (uint32_t ks = 0; ks < 4; ++ks) {
+            const uint64_t da_h = wg_desc_sw128(ah) + 2 * ks, da_l = wg_desc_sw128(al) + 2 * ks;
+            const uint64_t db_h = wg_desc_sw128(xh + brow + ks * 2048u), db_l = wg_desc_sw128(xl + brow + ks * 2048u);
+            wgmma_bf16<64, 1>(d[tp], da_h, db_h, (started || ks > 0) ? 1u : 0u);
+            if (kPasses == 3) {
+              wgmma_bf16<64, 1>(d[tp], da_l, db_h, 1u);
+              wgmma_bf16<64, 1>(d[tp], da_h, db_l, 1u);
+            }
+          }
+        }
+        wgmma_commit();
+        started = true;
       };
 
       fill_x(y0 - 1);
@@ -168,8 +191,11 @@ __global__ void __launch_bounds__(kWhThreads, 1) conv3x3_wgrad_halo_kernel(WgHal
       for (int i = 0; i < S; ++i) {
         fill_x(y0 + i + 1);
         fill_dy(y0 + i, 0);
+        mma(i, 0);
         fill_dy(y0 + i, 1);
+        mma(i, 1);
       }
+      xbase += S + 2;
     }
     // bias gradient partials: rows rsub + 32 i, summed over the 8 pixel-group threads of a row
 #pragma unroll
@@ -180,82 +206,28 @@ __global__ void __launch_bounds__(kWhThreads, 1) conv3x3_wgrad_halo_kernel(WgHal
       v += __shfl_xor_sync(0xffffffffu, v, 4);
       if (sub == 0) a.part_b[static_cast<long>(blockIdx.x) * 128 + rsub + 32 * i] = v;
     }
-  } else if (warp == 12) {
-    // ------------------------------------------------------------------ MMA issuer: the warp walks the loops, one elected lane
-    // issues (umma.cuh: elect_one_sync)
-    {
-      const bool leader = elect_one_sync();
-      const uint32_t idesc = umma_idesc_bf16(128, 64) | (1u << 16);          // B operand MN-major
-      const uint32_t xh = smem_u32(x_hi), xl = smem_u32(x_lo);
-      uint32_t xbase = 0, xwaited = 0, dcnt = 0;
-      bool started = false;
-      for (int u = 0; u < my_units; ++u) {
-        for (int i = 0; i < S; ++i) {
-          while (xwaited < xbase + i + 3) {       // input rows y-1, y, y+1 of output row i are ring entries xbase+i .. +2
-            mbar_wait(bars + WX_FULL + (xwaited & 3), (xwaited >> 2) & 1);
-            ++xwaited;
-          }
-          tc_fence_after();
-          for (int c = 0; c < 2; ++c, ++dcnt) {
-            const uint32_t buf = dcnt & 1;
-            mbar_wait(bars + WD_FULL + buf, (dcnt >> 1) & 1);
-            tc_fence_after();
-            const uint32_t ah = smem_u32(d_hi + buf * kWhDy), al = smem_u32(d_lo + buf * kWhDy);
-            for (int tp = 0; tp < a.ntaps; ++tp) {
-              const uint32_t slot = (xbase + i + 1 + a.tdy[tp]) & 3;
-              const uint32_t brow = (slot * kWhSeg + 1 + a.tdx[tp] + c * 64) * 128u;
-              const uint32_t d = tmem + tp * 64;
-#pragma unroll
-              for (uint32_t ks = 0; ks < 4; ++ks) {
-                const uint64_t da_h = umma_desc_sw128(ah) + 2 * ks, da_l = umma_desc_sw128(al) + 2 * ks;
-                const uint64_t db_h = umma_desc_sw128(xh + brow + ks * 2048u), db_l = umma_desc_sw128(xl + brow + ks * 2048u);
-                umma_bf16_if(leader, d, da_h, db_h, idesc, (started || ks > 0) ? 1u : 0u);
-                if (kPasses == 3) {
-                  umma_bf16_if(leader, d, da_l, db_h, idesc, 1u);
-                  umma_bf16_if(leader, d, da_h, db_l, idesc, 1u);
-                }
-              }
-            }
-            started = true;
-            umma_commit_if(leader, bars + WD_EMPTY + buf);
-          }
-          umma_commit_if(leader, bars + WX_EMPTY + ((xbase + i) & 3));      // input row y-1 is not needed below this output row
-        }
-        // the last two ring entries of the unit (rows y0+S-1, y0+S) are free once its MMAs have completed
-        umma_commit_if(leader, bars + WX_EMPTY + ((xbase + S) & 3));
-        umma_commit_if(leader, bars + WX_EMPTY + ((xbase + S + 1) & 3));
-        xbase += S + 2;
-      }
-      umma_commit_if(leader, bars + WH_DONE);
-    }
-  } else {
-    // ------------------------------------------------------------------ epilogue (once, at the end)
-    const int q = warp - 8;
+  }
+  operands_free();
+  // ---- drain: tap tp, output channel 64g + frag_row, input channel frag_col
+  {
     float* dst0 = a.part_w + static_cast<long>(blockIdx.x) * a.ntaps * 128 * 64;
     if (my_units > 0) {
-      mbar_wait_long(bars + WH_DONE, 0);
-      tc_fence_after();
-      for (int tp = 0; tp < a.ntaps; ++tp) {
-        float* dst = dst0 + (static_cast<long>(tp) * 128 + q * 32 + lane) * 64;
-        for (int cg = 0; cg < 2; ++cg) {
-          uint32_t raw[32];
-          tmem_ld32(tmem + (static_cast<uint32_t>(q * 32) << 16) + tp * 64 + cg * 32, raw);
-          tmem_ld_wait();
-          float4* o = reinterpret_cast<float4*>(dst + cg * 32);
+#pragma unroll
+      for (int tp = 0; tp < kWhMaxTaps; ++tp) {
+        if (tp >= a.ntaps) continue;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          float* dst = dst0 + (static_cast<long>(tp) * 128 + g * 64 + frag_row(t128, i)) * 64;
 #pragma unroll
           for (int j = 0; j < 8; ++j)
-            o[j] = make_float4(__uint_as_float(raw[4 * j]), __uint_as_float(raw[4 * j + 1]), __uint_as_float(raw[4 * j + 2]),
-                               __uint_as_float(raw[4 * j + 3]));
+            *reinterpret_cast<float2*>(dst + frag_col(t128, j, 0)) = make_float2(d[tp][4 * j + 2 * i], d[tp][4 * j + 2 * i + 1]);
         }
       }
     } else {
-      for (int i = threadIdx.x - 256; i < a.ntaps * 128 * 64; i += 128) dst0[i] = 0.f;
-      for (int i = threadIdx.x - 256; i < 128; i += 128) a.part_b[static_cast<long>(blockIdx.x) * 128 + i] = 0.f;
+      for (int i = threadIdx.x; i < a.ntaps * 128 * 64; i += kWhThreads) dst0[i] = 0.f;
+      for (int i = threadIdx.x; i < 128; i += kWhThreads) a.part_b[static_cast<long>(blockIdx.x) * 128 + i] = 0.f;
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 12) tmem_dealloc<512>(tmem);
 }
 
 __global__ void conv_wgrad_halo_reduce_kernel(const float* __restrict__ part_w, const float* __restrict__ part_b, int nparts,
@@ -277,9 +249,9 @@ __global__ void conv_wgrad_halo_reduce_kernel(const float* __restrict__ part_w, 
 
 extern "C" {
 
-// per CTA: 8 taps x 128 x 64 floats + 128 bias partials
+// per CTA: kWhMaxTaps taps x 128 x 64 floats + 128 bias partials
 size_t hg_conv3x3_wgrad_halo_workspace_bytes(void) {
-  return static_cast<size_t>(hg::num_sms()) * (8 * 128 * 64 + 128) * sizeof(float);
+  return static_cast<size_t>(hg::num_sms()) * (hg::kWhMaxTaps * 128 * 64 + 128) * sizeof(float);
 }
 
 // dw [ntaps, 128, 64] (rows >= nco and columns >= nci are zero), dbias [128] or null.  Requires W % 128 == 0.
@@ -290,7 +262,8 @@ int hg_conv3x3_wgrad_halo(const float* dy, const float* x, float* dw, float* dbi
   HG_REQUIRE(B > 0 && H > 0 && W > 0 && W % 128 == 0, "hg_conv3x3_wgrad_halo: the image width must be a multiple of 128 (got %d)", W);
   HG_REQUIRE(nco >= 1 && nco <= 128 && co0 >= 0 && co0 + nco <= Cout, "hg_conv3x3_wgrad_halo: bad output-channel block");
   HG_REQUIRE(nci >= 1 && nci <= 64 && ci0 >= 0 && ci0 + nci <= Cin, "hg_conv3x3_wgrad_halo: bad input-channel block");
-  HG_REQUIRE(ntaps >= 1 && ntaps <= 8, "hg_conv3x3_wgrad_halo: 1..8 taps per launch (8 x 64 TMEM columns)");
+  HG_REQUIRE(ntaps >= 1 && ntaps <= hg::kWhMaxTaps, "hg_conv3x3_wgrad_halo: 1..%d taps per launch (register accumulators)",
+             hg::kWhMaxTaps);
   HG_REQUIRE(passes == 1 || passes == 3, "hg_conv3x3_wgrad_halo: passes must be 1 or 3");
   HG_REQUIRE(((reinterpret_cast<uintptr_t>(dy) | reinterpret_cast<uintptr_t>(workspace) | reinterpret_cast<uintptr_t>(dw)) & 15) == 0,
              "hg_conv3x3_wgrad_halo: dy / dw / workspace must be 16-byte aligned");
@@ -308,7 +281,7 @@ int hg_conv3x3_wgrad_halo(const float* dy, const float* x, float* dw, float* dbi
   const int units = B * (W / 128) * (H / strip);
   const int grid = units < hg::num_sms() ? units : hg::num_sms();
   a.part_w = static_cast<float*>(workspace);
-  a.part_b = a.part_w + static_cast<size_t>(hg::num_sms()) * 8 * 128 * 64;
+  a.part_b = a.part_w + static_cast<size_t>(hg::num_sms()) * hg::kWhMaxTaps * 128 * 64;
   auto st = static_cast<cudaStream_t>(stream);
   cudaError_t e;
   if (passes == 3) {

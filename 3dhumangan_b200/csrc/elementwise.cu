@@ -1,11 +1,11 @@
 // bias_act and upfirdn2d: the two StyleGAN3 native ops the reference ships as CUDA plugins
 // (lib/components/ops/bias_act.cu:24-165, lib/components/ops/upfirdn2d.cu:29-375), rebuilt as
-// vectorised HBM-streaming kernels for sm_100a.  Both are bandwidth-bound (<= 10 FLOP/B).
+// vectorised HBM-streaming kernels for sm_90a.  Both are bandwidth-bound (<= 10 FLOP/B).
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <string.h>
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hg {
 
@@ -210,11 +210,11 @@ __global__ void __launch_bounds__(128) upfirdn2d_kernel(const float* __restrict_
 // g = filter flipped unless flip_filter (upfirdn2d.py:200-203), times sqrt(gain) per axis.
 // ---------------------------------------------------------------------------------------------------------------------
 //
-// Round-2 tuning (ncu: the first version was issue bound at 44 thread-instructions per output, 22 % of them FMAs):
+// Design (a first version was issue bound on index arithmetic and FMAs):
 //   * staging is ONE cp.async.bulk.tensor (TMA, 3-D box [1, TIH, PIN] of the [planes, H, W] tensor, out-of-bounds = zero fill =
 //     the padding) per tile instead of ~1 500 4-byte cp.async with their bounds checks (used when W % 4 == 0 and x is
 //     16-byte aligned; the cp.async path is kept for everything else);
-//   * the vertical pass runs on column PAIRS with FFMA2 (sm_100 packed fp32): half the FMA instructions;
+//   * the vertical pass runs on column PAIRS (float2 arithmetic, one pair per tap);
 //   * a horizontal item makes 8 outputs from float4-aligned window reads, so its index arithmetic is amortised twice as far.
 template <int T, bool kUp>
 struct SepGeom {
@@ -226,8 +226,8 @@ struct SepGeom {
   static constexpr int NV2 = T + 2;                                   // down, 2 outputs (vertical pass)
   static constexpr int TIW = kUp ? TOW / 2 + T / 2 + 1 : 2 * TOW + T - 2;
   static constexpr int TIH = kUp ? TOH / 2 + T / 2 + 1 : 2 * TOH + T - 2;
-  // staged row: the tile may start up to 3 columns early (a TMA box must start on a 16-byte boundary of the row:
-  // tools/experiments/tma_probe.cu -- an unaligned innermost coordinate is an illegal-instruction fault)
+  // staged row: the tile may start up to 3 columns early, so that the innermost coordinate of every TMA box is a multiple
+  // of 4 floats (16 bytes)
   static constexpr int PIN = (TIW + 3 + 3) & ~3;
   static constexpr int PMID = TOW + 4;
   static constexpr int IN_BYTES = TIH * PIN * 4;
@@ -282,7 +282,7 @@ __device__ __forceinline__ void sep_fir4(const float* __restrict__ v, const floa
   }
 }
 
-// the same on two adjacent columns at once (FFMA2): v[j] = (column c, column c+1) of window row j
+// the same on two adjacent columns at once (float2): v[j] = (column c, column c+1) of window row j
 template <int T, bool kUp, int NQ>
 __device__ __forceinline__ void sep_fir_pair(const float2* __restrict__ v, const float* __restrict__ g, bool odd, float2 (&o)[NQ]) {
 #pragma unroll
@@ -292,19 +292,19 @@ __device__ __forceinline__ void sep_fir_pair(const float2* __restrict__ v, const
 #pragma unroll
       for (int t = 0; t < T / 2; ++t) {
         const float2 ge = make_float2(g[2 * t], g[2 * t]), go = make_float2(g[2 * t + 1], g[2 * t + 1]);
-        o[0] = __ffma2_rn(ge, v[t], o[0]);
-        o[1] = __ffma2_rn(go, v[t + 1], o[1]);
-        o[2] = __ffma2_rn(ge, v[t + 1], o[2]);
-        o[3] = __ffma2_rn(go, v[t + 2], o[3]);
+        o[0] = ffma2(ge, v[t], o[0]);
+        o[1] = ffma2(go, v[t + 1], o[1]);
+        o[2] = ffma2(ge, v[t + 1], o[2]);
+        o[3] = ffma2(go, v[t + 2], o[3]);
       }
     } else {
 #pragma unroll
       for (int t = 0; t < T / 2; ++t) {
         const float2 ge = make_float2(g[2 * t], g[2 * t]), go = make_float2(g[2 * t + 1], g[2 * t + 1]);
-        o[0] = __ffma2_rn(go, v[t], o[0]);
-        o[1] = __ffma2_rn(ge, v[t], o[1]);
-        o[2] = __ffma2_rn(go, v[t + 1], o[2]);
-        o[3] = __ffma2_rn(ge, v[t + 1], o[3]);
+        o[0] = ffma2(go, v[t], o[0]);
+        o[1] = ffma2(ge, v[t], o[1]);
+        o[2] = ffma2(go, v[t + 1], o[2]);
+        o[3] = ffma2(ge, v[t + 1], o[3]);
       }
     }
   } else {
@@ -312,7 +312,7 @@ __device__ __forceinline__ void sep_fir_pair(const float2* __restrict__ v, const
     for (int k = 0; k < T; ++k) {
       const float2 gk = make_float2(g[k], g[k]);
 #pragma unroll
-      for (int q = 0; q < NQ; ++q) o[q] = __ffma2_rn(gk, v[2 * q + k], o[q]);
+      for (int q = 0; q < NQ; ++q) o[q] = ffma2(gk, v[2 * q + k], o[q]);
     }
   }
 }
@@ -342,8 +342,8 @@ __device__ __forceinline__ void sep_hpass(const float* __restrict__ in_s, float*
     }
   } else {
     // y[q] = sum_k g[k] * w[SH + 2q + k]: with the window read as pairs W2[i] = (w[2i], w[2i+1]) and the taps as pairs
-    // G2[j] = (g'[M0 + 2j], g'[M0 + 2j + 1]), g'[m] = g[m - SH] (0 outside), M0 = SH & ~1, it is one FFMA2 per tap PAIR and
-    // a final x + y: half the FMA instructions, all register pairs naturally aligned.
+    // G2[j] = (g'[M0 + 2j], g'[M0 + 2j + 1]), g'[m] = g[m - SH] (0 outside), M0 = SH & ~1, it is one ffma2 per tap PAIR and
+    // a final x + y, all register pairs naturally aligned.
     constexpr int M0 = SH & ~1, NP = T / 2 + (SH & 1);
     static_assert(2 * (7 + M0 / 2 + NP) <= NW, "pair window");
     float2 G2[NP];
@@ -354,8 +354,7 @@ __device__ __forceinline__ void sep_hpass(const float* __restrict__ in_s, float*
     }
     // item -> (column group a, row r) with r FASTEST: the 8 threads of an LDS.128 phase then read 8 consecutive rows (pitch
     // 148 floats = 20 banks apart: conflict-free); with the column group fastest their windows start 16 floats apart -- two
-    // bank groups for 8 threads, a 4-way conflict on every window load (ncu: 64 % of the samples waiting on shared memory,
-    // issue slots 27 % busy)
+    // bank groups for 8 threads, a 4-way conflict on every window load
     for (int i = tid; i < NITEMS; i += G::THREADS) {
       const int a = i / G::TIH, r = i - a * G::TIH;
       const float* wsrc = in_s + r * G::PIN + 16 * a;
@@ -369,9 +368,9 @@ __device__ __forceinline__ void sep_hpass(const float* __restrict__ in_s, float*
       float o[8];
 #pragma unroll
       for (int q = 0; q < 8; ++q) {
-        float2 acc = __fmul2_rn(G2[0], W2[q + M0 / 2]);
+        float2 acc = fmul2(G2[0], W2[q + M0 / 2]);
 #pragma unroll
-        for (int j = 1; j < NP; ++j) acc = __ffma2_rn(G2[j], W2[q + M0 / 2 + j], acc);
+        for (int j = 1; j < NP; ++j) acc = ffma2(G2[j], W2[q + M0 / 2 + j], acc);
         o[q] = acc.x + acc.y;
       }
       float4* m4 = reinterpret_cast<float4*>(mid + r * G::PMID + 8 * a);
@@ -491,7 +490,7 @@ __global__ void __launch_bounds__(SepGeom<T, kUp>::THREADS, kUp ? 1 : 2) upfirdn
       default: sep_hpass<T, kUp, 3>(in_s, mid, g, oddx, tid); break;
     }
     __syncthreads();
-    // ---- (3) vertical: item = (group of 4 output columns, group of NQ output rows) on two column pairs (FFMA2): float4
+    // ---- (3) vertical: item = (group of 4 output columns, group of NQ output rows) on two column pairs (float2): float4
     //      columns of `mid`, float4 stores (rows of the output are 16-byte aligned when outW % 4 == 0)
     constexpr int NQ = kUp ? 4 : 2;                   // 16 x 16 items (up, 64 rows) / 16 x 16 items (down, 32 rows)
     constexpr int NW = kUp ? G::NV : G::NV2;

@@ -300,17 +300,16 @@ __global__ void __launch_bounds__(kGeoThreads, 1) geo_kernel(GeoArgs a) {
 #pragma unroll 4
       for (int v = 0; v < Vn; ++v) consider(sv[v]);
     } else {
-      // two vertices per step on packed fp32 (FFMA2 / FMUL2 / FADD2 lanes are the same IEEE operations as the scalar ones:
+      // two vertices per step on fp32 pairs (ffma2 / fmul2 / fadd2 are the same IEEE operations as the scalar ones:
       // p - q as fma(q, -1, p) rounds the exact difference once, like the subtraction; products and sums are NOT contracted),
       // candidates still examined in index order: bit-identical distances and the same tie-breaking as `consider`
       const float2 px2 = make_float2(px, px), py2 = make_float2(py, py), pz2 = make_float2(pz, pz), neg1 = make_float2(-1.f, -1.f);
       auto consider2 = [&](const float4 xy, const float4 zw) {
-        const float2 ex = __ffma2_rn(make_float2(xy.x, xy.y), neg1, px2);
-        const float2 ey = __ffma2_rn(make_float2(xy.z, xy.w), neg1, py2);
-        const float2 ez = __ffma2_rn(make_float2(zw.x, zw.y), neg1, pz2);
-        // ptxas fuses mul.rn.f32x2 + add.rn.f32x2 into FFMA2 (it never does that to the scalar .rn forms): the products go
-        // through an opaque register so that they are rounded before the sums, as in the oracle
-        const float2 d2 = __fadd2_rn(__fadd2_rn(keep2(__fmul2_rn(ex, ex)), keep2(__fmul2_rn(ey, ey))), keep2(__fmul2_rn(ez, ez)));
+        const float2 ex = ffma2(make_float2(xy.x, xy.y), neg1, px2);
+        const float2 ey = ffma2(make_float2(xy.z, xy.w), neg1, py2);
+        const float2 ez = ffma2(make_float2(zw.x, zw.y), neg1, pz2);
+        // the products go through an opaque register so that they are rounded before the sums, as in the oracle
+        const float2 d2 = fadd2(fadd2(keep2(fmul2(ex, ex)), keep2(fmul2(ey, ey))), keep2(fmul2(ez, ez)));
         const int v0 = __float_as_int(zw.z), v1 = __float_as_int(zw.w);
         if (d2.x < best || (d2.x == best && v0 < bi)) { best = d2.x; bi = v0; }
         if (d2.y < best || (d2.y == best && v1 < bi)) { best = d2.y; bi = v1; }

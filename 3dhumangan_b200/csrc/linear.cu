@@ -1,14 +1,14 @@
-// Weight packing + the generic row-major linear layer  Y[M,N] = X[M,K] . W[N,K]^T + b  on tcgen05.
+// Weight packing + the generic row-major linear layer  Y[M,N] = X[M,K] . W[N,K]^T + b  on wgmma.
 //
 // Used for (a) the low-resolution SPADE style projections (SURVEY.md §8a a13: W_s . feature_maps
 // is linear, so it commutes with the bilinear up-sample and runs at render resolution), and
-// (b) as the smallest complete user of the tensor-core primitives in umma.cuh (self-test target).
+// (b) as the smallest complete user of the tensor-core primitives in wgmma.cuh (self-test target).
 //
 // Precision modes: passes == 1  plain bf16 operands, fp32 accumulate;
 //                  passes == 3  bf16x3 split (A_hi.B_hi + A_lo.B_hi + A_hi.B_lo), ~2^-16 relative,
 //                               the mode that meets the 1e-3-of-fp32 parity contract.
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hg {
 
@@ -45,61 +45,48 @@ __global__ void pack_weight_kernel(const float* __restrict__ W, int N, int K, in
 }
 
 // ------------------------------------------------------------------------------------------
-// linear kernel
+// linear kernel: warps 0-7 are two warpgroups; warpgroup g loads rows 64g..64g+63 of the X tile, issues the wgmmas of those
+// rows (accumulator [64 x N] in registers) and stores them; warp 8 streams the weight tiles.
 // ------------------------------------------------------------------------------------------
-constexpr int kLinThreads = 320;  // warps 0-7: load X / epilogue, warp 8: MMA issuer, warp 9: weight producer
+constexpr int kLinThreads = 288;
 constexpr int kLinStages = 3;
 constexpr uint32_t kChunkBytesA = 128 * 128;  // one [128 x 64] bf16 tile
 constexpr uint32_t kStageBytesB = 256 * 128;  // one [256 x 64] bf16 tile (max)
 constexpr uint32_t kLinSmem = 8 * kChunkBytesA + kLinStages * kStageBytesB + 256 + 1024;
 
-template <int kPasses>
+template <int kPasses, int N>
 __global__ void __launch_bounds__(kLinThreads, 1)
 linear_kernel(const float* __restrict__ X, int ldx, int M, int K, const uint8_t* __restrict__ Wimg, int Nb,
-              int nblocks, int N, const float* __restrict__ bias, float* __restrict__ Y, int ldy) {
+              int nblocks, int N_, const float* __restrict__ bias, float* __restrict__ Y, int ldy) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* a_hi = smem;
   uint8_t* a_lo = smem + 4 * kChunkBytesA;
   uint8_t* b_st = smem + 8 * kChunkBytesA;
   uint64_t* bars = reinterpret_cast<uint64_t*>(b_st + kLinStages * kStageBytesB);
-  uint64_t* a_full = bars + 0;
-  uint64_t* a_empty = bars + 1;
-  uint64_t* b_full = bars + 2;                  // [kLinStages]
-  uint64_t* b_empty = bars + 2 + kLinStages;    // [kLinStages]
-  uint64_t* acc_full = bars + 2 + 2 * kLinStages;   // [2]
-  uint64_t* acc_empty = bars + 4 + 2 * kLinStages;  // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 6 + 2 * kLinStages);
+  uint64_t* b_full = bars;                      // [kLinStages]
+  uint64_t* b_empty = bars + kLinStages;        // [kLinStages]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int kchunks = (K + 63) / 64;
   const int num_tiles = (M + 127) / 128;
 
   if (threadIdx.x == 0) {
-    mbar_init(a_full, 256);
-    mbar_init(a_empty, 1);
     for (int i = 0; i < kLinStages; ++i) {
       mbar_init(b_full + i, 1);
-      mbar_init(b_empty + i, 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(acc_full + i, 1);
-      mbar_init(acc_empty + i, 8);
+      mbar_init(b_empty + i, 2);     // one arrival per warpgroup
     }
     fence_mbar_init();
   }
-  if (warp == 8) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
 
   if (warp < 8) {
-    // ------------------------------------------------------------ X loader + epilogue
-    uint32_t acc_use = 0, it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      mbar_wait(a_empty, (it & 1) ^ 1);
-      for (int r = warp; r < 128; r += 8) {
+    const int g = warp >> 2, t = threadIdx.x & 127;
+    const uint32_t a_off = g * 64 * 128;           // this warpgroup's rows inside every [128 x 64] chunk
+    uint32_t st = 0, ph = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      // ------------------------------------------------------------ X rows 64g.. -> A (the previous tile's wgmmas are done)
+      for (int r = g * 64 + (warp & 3); r < g * 64 + 64; r += 4) {
         const long grow = static_cast<long>(tile) * 128 + r;
         for (int kb = lane * 8; kb < kchunks * 64; kb += 256) {
           float x[8];
@@ -122,66 +109,49 @@ linear_kernel(const float* __restrict__ X, int ldx, int M, int K, const uint8_t*
         }
       }
       fence_proxy_async_smem();
-      mbar_arrive(a_full);
+      named_barrier(1 + g, 128);
 
-      const int q = warp & 3, h = warp >> 2;
-      const int row = q * 32 + lane;
-      const long grow = static_cast<long>(tile) * 128 + row;
-      for (int nb = 0; nb < nblocks; ++nb, ++acc_use) {
-        const uint32_t buf = acc_use & 1;
-        mbar_wait(acc_full + buf, (acc_use >> 1) & 1);
-        tc_fence_after();
-        for (int c0 = h * 32; c0 < Nb; c0 += 64) {
-          uint32_t v[32];
-          tmem_ld32(tmem + (static_cast<uint32_t>(q * 32) << 16) + buf * 256 + c0, v);
-          tmem_ld_wait();
-          if (grow < M) {
+      for (int nb = 0; nb < nblocks; ++nb) {
+        float d[N / 2];
+        // one weight stage: wait, issue, and release the stage consumed one step earlier once its wgmmas are done
+        uint32_t prev = ~0u;
+        auto stage = [&](uint32_t a_tile, uint32_t a_tile2, bool two, bool accumulate) {
+          mbar_wait(b_full + st, ph);
+          acc_fence(d);
+          wgmma_fence();
+          const uint32_t bt = smem_u32(b_st + st * kStageBytesB);
+          wg_k64<N>(d, a_tile, bt, accumulate);
+          if (two) wg_k64<N>(d, a_tile2, bt, true);
+          wgmma_commit();
+          wgmma_wait<1>();
+          acc_fence(d);
+          if (prev != ~0u && t == 0) mbar_arrive(b_empty + prev);
+          prev = st;
+          if (++st == kLinStages) { st = 0; ph ^= 1; }
+        };
+        for (int kc = 0; kc < kchunks; ++kc) {
+          const uint32_t ahi = smem_u32(a_hi + kc * kChunkBytesA) + a_off, alo = smem_u32(a_lo + kc * kChunkBytesA) + a_off;
+          stage(ahi, alo, kPasses == 3, kc > 0);
+          if (kPasses == 3) stage(ahi, ahi, false, true);
+        }
+        wgmma_wait<0>();
+        acc_fence(d);
+        if (t == 0) mbar_arrive(b_empty + prev);
+        // ---------------------------------------------------------- epilogue straight from the fragments
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const int n = nb * Nb + c0 + j;
-              if (n < N) Y[grow * ldy + n] = __uint_as_float(v[j]) + (bias ? bias[n] : 0.f);
+        for (int i = 0; i < 2; ++i) {
+          const long grow = static_cast<long>(tile) * 128 + g * 64 + frag_row(t, i);
+          if (grow >= M) continue;
+#pragma unroll
+          for (int j = 0; j < N / 8; ++j)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int c = frag_col(t, j, e), n = nb * Nb + c;
+              if (c < Nb && n < N_) Y[grow * ldy + n] = d[4 * j + 2 * i + e] + (bias ? bias[n] : 0.f);
             }
-          }
         }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(acc_empty + buf);
       }
-    }
-  } else if (warp == 8) {
-    // ------------------------------------------------------------ MMA issuer
-    {      // the warp walks the loops, one elected lane issues (umma.cuh: elect_one_sync)
-      const bool leader = elect_one_sync();
-      const uint32_t idesc = umma_idesc_bf16(128, Nb);
-      uint32_t st = 0, ph = 0, acc_use = 0, it = 0;
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-        mbar_wait(a_full, it & 1);
-        tc_fence_after();
-        for (int nb = 0; nb < nblocks; ++nb, ++acc_use) {
-          const uint32_t buf = acc_use & 1;
-          mbar_wait(acc_empty + buf, ((acc_use >> 1) & 1) ^ 1);
-          tc_fence_after();
-          const uint32_t d = tmem + buf * 256;
-          for (int kc = 0; kc < kchunks; ++kc) {
-            mbar_wait(b_full + st, ph);
-            tc_fence_after();
-            umma_k64_if(leader, d, smem_u32(a_hi + kc * kChunkBytesA), smem_u32(b_st + st * kStageBytesB), idesc, kc > 0);
-            if (kPasses == 3)
-              umma_k64_if(leader, d, smem_u32(a_lo + kc * kChunkBytesA), smem_u32(b_st + st * kStageBytesB), idesc, true);
-            umma_commit_if(leader, b_empty + st);
-            if (++st == kLinStages) { st = 0; ph ^= 1; }
-            if (kPasses == 3) {
-              mbar_wait(b_full + st, ph);
-              tc_fence_after();
-              umma_k64_if(leader, d, smem_u32(a_hi + kc * kChunkBytesA), smem_u32(b_st + st * kStageBytesB), idesc, true);
-              umma_commit_if(leader, b_empty + st);
-              if (++st == kLinStages) { st = 0; ph ^= 1; }
-            }
-          }
-          umma_commit_if(leader, acc_full + buf);
-        }
-        umma_commit_if(leader, a_empty);
-      }
+      named_barrier(1 + g, 128);     // every warp of the group is done reading before the next tile overwrites A
     }
   } else {
     // ------------------------------------------------------------ weight producer (bulk copies from L2)
@@ -202,9 +172,15 @@ linear_kernel(const float* __restrict__ X, int ldx, int M, int K, const uint8_t*
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 8) tmem_dealloc<512>(tmem);
+}
+
+template <int kPasses, int N>
+static int launch_linear(int grid, cudaStream_t st, const float* X, int ldx, int M, int K, const uint8_t* img, int Nb, int nblocks,
+                         int N_, const float* bias, float* Y, int ldy) {
+  const cudaError_t e = cudaFuncSetAttribute(linear_kernel<kPasses, N>, cudaFuncAttributeMaxDynamicSharedMemorySize, kLinSmem);
+  if (e != cudaSuccess) { set_error("hg_linear: smem opt-in failed: %s", cudaGetErrorString(e)); return 2; }
+  linear_kernel<kPasses, N><<<grid, kLinThreads, kLinSmem, st>>>(X, ldx, M, K, img, Nb, nblocks, N_, bias, Y, ldy);
+  return check_launch("hg_linear");
 }
 
 }  // namespace hg
@@ -246,17 +222,15 @@ int hg_linear(const float* X, int ldx, int M, int K, const void* Wimg, int Nb, i
   const int grid = num_tiles < hg::num_sms() ? num_tiles : hg::num_sms();
   auto st = static_cast<cudaStream_t>(stream);
   const auto* img = static_cast<const uint8_t*>(Wimg);
-  cudaError_t e;
+  // wgmma N: the smallest of 64 / 128 / 256 that covers a block (columns past Nb are computed and dropped)
   if (passes == 3) {
-    e = cudaFuncSetAttribute(hg::linear_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, hg::kLinSmem);
-    if (e != cudaSuccess) { hg::set_error("hg_linear: smem opt-in failed: %s", cudaGetErrorString(e)); return 2; }
-    hg::linear_kernel<3><<<grid, hg::kLinThreads, hg::kLinSmem, st>>>(X, ldx, M, K, img, Nb, nblocks, N, bias, Y, ldy);
-  } else {
-    e = cudaFuncSetAttribute(hg::linear_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, hg::kLinSmem);
-    if (e != cudaSuccess) { hg::set_error("hg_linear: smem opt-in failed: %s", cudaGetErrorString(e)); return 2; }
-    hg::linear_kernel<1><<<grid, hg::kLinThreads, hg::kLinSmem, st>>>(X, ldx, M, K, img, Nb, nblocks, N, bias, Y, ldy);
+    if (Nb <= 64) return hg::launch_linear<3, 64>(grid, st, X, ldx, M, K, img, Nb, nblocks, N, bias, Y, ldy);
+    if (Nb <= 128) return hg::launch_linear<3, 128>(grid, st, X, ldx, M, K, img, Nb, nblocks, N, bias, Y, ldy);
+    return hg::launch_linear<3, 256>(grid, st, X, ldx, M, K, img, Nb, nblocks, N, bias, Y, ldy);
   }
-  return hg::check_launch("hg_linear");
+  if (Nb <= 64) return hg::launch_linear<1, 64>(grid, st, X, ldx, M, K, img, Nb, nblocks, N, bias, Y, ldy);
+  if (Nb <= 128) return hg::launch_linear<1, 128>(grid, st, X, ldx, M, K, img, Nb, nblocks, N, bias, Y, ldy);
+  return hg::launch_linear<1, 256>(grid, st, X, ldx, M, K, img, Nb, nblocks, N, bias, Y, ldy);
 }
 
 }  // extern "C"

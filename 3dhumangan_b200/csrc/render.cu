@@ -6,38 +6,36 @@
 //   vr.ray_integration              lib/generators/volume_rendering.py:12-56
 //   the [B,N,F+4] / [B,N,256..512] intermediates of Map3DGenerator.render (map3d_generator.py:427-515)
 //
-// A CTA owns tiles of 128 sample points = (128/S) whole rays.  The eight GEMM steps of the MLP run
-// back to back on tcgen05 with the activations never leaving the SM: accumulator (TMEM) ->
-// sin(F*acc + P) in registers -> bf16 hi/lo operand in shared memory -> next tcgen05.mma, while the
-// weight tiles stream from L2 through the bulk-copy engine.  FiLM frequency/phase, bias and the
-// x30 of the sine layers are folded into one (F, P) table per layer and sample (host side).  The
-// sigma and rgb heads are dot products on the fp32 activations; transmittance is a per-ray scan in
-// shared memory and the weighted feature sum is a warp shuffle transpose-reduce, so that only
-// [rays, 256 feat + 3 rgb + depth] ever reaches HBM.
+// A CTA owns tiles of 128 sample points = (128/S) whole rays; warpgroup g owns points 64g..64g+63 and runs the MLP for them
+// on wgmma with the activations never leaving the SM (accumulator -> sin(F*acc + P) -> bf16 hi/lo operand -> next wgmma),
+// while warp 8 streams the weight tiles from L2.  FiLM frequency/phase, bias and the x30 of the sine layers are folded into
+// one (F, P) table per layer and sample (host side); only [rays, 256 feat + 3 rgb + depth] ever reaches HBM.
 //
-// Layer schedule per tile (acc A = TMEM cols 0..255, acc B = cols 256..511):
-//   L0   rec[K=64: xyz*s, geo31, 0]  x W01(coord | geo)      -> A (coord pre-act), B (geo pre-act)
-//   E0   a = sin(30*(A+b))                                    -> operand
-//   L1a  a x Wn0[:, 0:256]                                    -> A
-//   E1   g = sin(30*(B+b))                                    -> operand
-//   L1b  g x Wn0[:, 256:512]                                  -> A (accumulate)
-//   E2..E4  x = sin(F*(acc+b)+P) ; L: network.1..3            -> B, A, B
-//   E5   x4 (+ sigma head) ; L: color_layer_sine[:, 3:]       -> A       (view-direction term in P)
-//   E6   c (+ rgb head)    ; L: feature_layer_linear          -> B
+// Layer schedule per tile (one [64 x 256] fp32 accumulator per warpgroup; the weight blob holds the stages in this order):
+//   L0c  rec[K=64: xyz*s, geo31, 0] x W01(coord)               -> acc -> kept in per-thread local memory (coord pre-act)
+//   L0g  rec x W01(geo)                                         -> acc
+//   E1   g = sin(30*(acc+b))                                    -> operand
+//   L1b  g x Wn0[:, 256:512]                                    -> acc
+//   E0   a = sin(30*(coord pre-act + b))                        -> operand
+//   L1a  a x Wn0[:, 0:256]                                      -> acc (accumulate)
+//   E2..E4  x = sin(F*(acc+b)+P) ; L: network.1..3             -> acc
+//   E5   x4 (+ sigma head) ; L: color_layer_sine[:, 3:]        -> acc       (view-direction term in P)
+//   E6   c (+ rgb head)    ; L: feature_layer_linear           -> acc
 //   E7   feat + compositing
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hg {
 
 constexpr int kRH = 256;           // hidden_dim == feature_dim
-constexpr int kRenThreads = 320;   // warps 0-7 rows, 8 MMA, 9 weight producer
+constexpr int kRenThreads = 384;   // warpgroups 0-1 rows, warp 8 weight producer
 constexpr int kRenStages = 2;
 constexpr uint32_t kRA = 128 * 128;   // operand chunk [128 x 64] bf16
 constexpr uint32_t kRB = 256 * 128;   // weight stage  [256 x 64] bf16
 constexpr int kFilmLayers = 7;        // coord, geo, network.0..3, color
 constexpr int kWeightStages = 60;     // per tile, hi+lo (see schedule above)
 constexpr int kRayOut = 260;          // floats per ray: 256 feat, 3 rgb, depth
+constexpr int kScr = 65;              // row stride (floats) of the compositing scratch
 
 struct RenderArgs {
   const float* rec;      // [B,N,36] point records (geo.cu)
@@ -65,16 +63,15 @@ struct RenSmem {
   float* w_sigma;  // [256]
   float* w_rgb;    // [3][256]
   float* b_feat;   // [256]
-  float* part;     // [2][128][4] sigma / rgb partial dots per column half
+  float* part;     // [128][4] sigma / rgb dots per point
   float* tr;       // [128] 1 - alpha + 1e-12
   float* wgt;      // [128] compositing weights
   float* zs;       // [128]
   float* rayw;     // [128] per-ray sum of weights (first rays_per_tile entries)
   uint64_t* bars;
-  uint32_t* tmem_slot;
 };
-constexpr uint32_t kRenFloats = kFilmLayers * 2 * kRH + kRH + 3 * kRH + kRH + 2 * 128 * 4 + 4 * 128;
-constexpr uint32_t kRenSmemBytes = 8 * kRA + kRenStages * kRB + kRenFloats * 4 + 16 * 8 + 16 + 1024;
+constexpr uint32_t kRenFloats = kFilmLayers * 2 * kRH + kRH + 3 * kRH + kRH + 128 * 4 + 4 * 128;
+constexpr uint32_t kRenSmemBytes = 8 * kRA + kRenStages * kRB + kRenFloats * 4 + 16 * 8 + 1024;
 
 __device__ __forceinline__ RenSmem ren_carve(uint8_t* raw) {
   uint8_t* s = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~uintptr_t(1023));
@@ -87,18 +84,17 @@ __device__ __forceinline__ RenSmem ren_carve(uint8_t* raw) {
   m.w_sigma = f; f += kRH;
   m.w_rgb = f; f += 3 * kRH;
   m.b_feat = f; f += kRH;
-  m.part = f; f += 2 * 128 * 4;
+  m.part = f; f += 128 * 4;
   m.tr = f; f += 128;
   m.wgt = f; f += 128;
   m.zs = f; f += 128;
   m.rayw = f; f += 128;
   m.bars = reinterpret_cast<uint64_t*>(f);
-  m.tmem_slot = reinterpret_cast<uint32_t*>(m.bars + 16);
   return m;
 }
-enum { RA_FULL = 0 /*4*/, RB_FULL = 4 /*2*/, RB_EMPTY = 6 /*2*/, RL_FULL = 8 };
+enum { RB_FULL = 0 /*2*/, RB_EMPTY = 2 /*2*/ };
 
-__device__ __forceinline__ void ren_rows_barrier() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+__device__ __forceinline__ void ren_rows_barrier() { named_barrier(1, 256); }
 
 // sin(t) for |t| up to a few thousand: two-term Cody-Waite reduction by 2*pi, then the SFU sine on
 // [-pi, pi] (abs error ~2^-21).  The reference path evaluates torch.sin on fp32 tensors.
@@ -110,122 +106,91 @@ __device__ __forceinline__ float sin_reduced(float t) {
   return __sinf(r);
 }
 
-// the same evaluation on a pair (packed fp32 for everything in front of the SFU: identical operations, half the instructions)
+// the same evaluation on a pair
 __device__ __forceinline__ float2 sin_reduced2(float2 t) {
-  const float2 y = __fmul2_rn(t, make_float2(0.15915494309189535f, 0.15915494309189535f));
+  const float2 y = fmul2(t, make_float2(0.15915494309189535f, 0.15915494309189535f));
   const float2 big = make_float2(12582912.f, 12582912.f), nbig = make_float2(-12582912.f, -12582912.f);
-  const float2 k = __fadd2_rn(__fadd2_rn(y, big), nbig);
-  float2 r = __ffma2_rn(k, make_float2(-6.2831854820251465f, -6.2831854820251465f), t);
-  r = __ffma2_rn(k, make_float2(1.7484555314695172e-07f, 1.7484555314695172e-07f), r);
+  const float2 k = fadd2(fadd2(y, big), nbig);
+  float2 r = ffma2(k, make_float2(-6.2831854820251465f, -6.2831854820251465f), t);
+  r = ffma2(k, make_float2(1.7484555314695172e-07f, 1.7484555314695172e-07f), r);
   return make_float2(__sinf(r.x), __sinf(r.y));
 }
 
-__device__ __forceinline__ float transpose_reduce32r(float (&v)[32], int lane) {
-#pragma unroll
-  for (int w = 16; w >= 1; w >>= 1) {
-    const bool upper = (lane & w) != 0;
-#pragma unroll
-    for (int i = 0; i < w; ++i) {
-      const float send = upper ? v[i] : v[i + w];
-      const float keep = upper ? v[i + w] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, w);
-    }
-  }
-  return v[0];
+// two consecutive-k fp32 values (k even) of one row -> the hi (and lo) operand tiles
+template <bool kSplit>
+__device__ __forceinline__ void store_a2(uint8_t* tile_hi, uint8_t* tile_lo, uint32_t row, uint32_t k, float x0, float x1) {
+  uint32_t h, l;
+  split_bf16x2(x0, x1, h, l);
+  const uint32_t off = sw128_offset(row, k);
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(smem_u32(tile_hi) + off), "r"(h));
+  if (kSplit) asm volatile("st.shared.b32 [%0], %1;" ::"r"(smem_u32(tile_lo) + off), "r"(l));
 }
 
-template <int kPasses>
-__device__ __forceinline__ void ren_mma_chunk(const RenSmem& m, bool leader, uint32_t& st, uint32_t& ph, uint32_t tmem_d,
-                                              uint32_t a_hi, uint32_t a_lo, uint32_t idesc, bool accumulate) {
-  mbar_wait(m.bars + RB_FULL + st, ph);
-  tc_fence_after();
-  umma_k64_if(leader, tmem_d, a_hi, smem_u32(m.b_st + st * kRB), idesc, accumulate);
-  if (kPasses == 3) umma_k64_if(leader, tmem_d, a_lo, smem_u32(m.b_st + st * kRB), idesc, true);
-  umma_commit_if(leader, m.bars + RB_EMPTY + st);
-  if (++st == kRenStages) { st = 0; ph ^= 1; }
-  if (kPasses == 3) {
-    mbar_wait(m.bars + RB_FULL + st, ph);
-    tc_fence_after();
-    umma_k64_if(leader, tmem_d, a_hi, smem_u32(m.b_st + st * kRB), idesc, true);
-    umma_commit_if(leader, m.bars + RB_EMPTY + st);
-    if (++st == kRenStages) { st = 0; ph ^= 1; }
-  }
+// per-thread spill slot of one accumulator (the coord pre-activation waits there while the geo half of network.0 runs)
+__device__ __forceinline__ void stash_store(float* slot, const float (&d)[128]) {
+  const uint32_t base = static_cast<uint32_t>(__cvta_generic_to_local(slot));
+#pragma unroll
+  for (int i = 0; i < 128; i += 4)
+    asm volatile("st.local.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(base + i * 4), "f"(d[i]), "f"(d[i + 1]), "f"(d[i + 2]), "f"(d[i + 3])
+                 : "memory");
+}
+__device__ __forceinline__ float4 stash_load4(const float* slot, int i) {
+  float4 v;
+  asm volatile("ld.local.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w)
+               : "r"(static_cast<uint32_t>(__cvta_generic_to_local(slot)) + i * 4)
+               : "memory");
+  return v;
 }
 
-// Activation epilogue of one layer: TMEM accumulator -> x = sin(F*acc + P) -> bf16 hi/lo operand.
-// kHead: 0 none, 1 sigma dot (1 value), 2 rgb dots (3 values) accumulated into part[h][row][*].
-template <int kPasses, int kHead>
-__device__ __forceinline__ void film_epilogue(const RenSmem& m, uint32_t tmem_acc, int layer, int warp, int lane,
-                                              bool defer_arrive) {
-  const int q = warp & 3, h = warp >> 2;
-  const int row = q * 32 + lane;
+// Activation epilogue of one layer for warpgroup g: accumulator fragments -> x = sin(F*acc + P) -> bf16 hi/lo operand.
+// kHead: 0 none, 1 sigma dot (1 value), 2 rgb dots (3 values) of each point -> part[row][*].  kStash: the fragments come
+// from the per-thread stash instead of `d` (which is left untouched).
+template <int kPasses, int kHead, bool kStash = false>
+__device__ __forceinline__ void film_epilogue(const RenSmem& m, const float (&d)[128], const float* stash, int layer, int g, int t) {
   uint32_t F = smem_u32(m.film + (layer * 2 + 0) * kRH);
   uint32_t P = smem_u32(m.film + (layer * 2 + 1) * kRH);
   opaque(F);   // the per-sample FiLM table is refreshed between tiles: table loads stay inside this call
   opaque(P);
-  uint32_t wsig = smem_u32(m.w_sigma), wrgb = smem_u32(m.w_rgb);
-  opaque(wsig);
-  opaque(wrgb);
-  float d0 = 0.f, d1 = 0.f, d2 = 0.f;
-#pragma unroll 1
-  for (int kc = 0; kc < 4; ++kc) {
-    const int c0 = kc * 64 + h * 32;
-    uint32_t raw[32];
-    tmem_ld32(tmem_acc + (static_cast<uint32_t>(q * 32) << 16) + c0, raw);
-    tmem_ld_wait();
+  float dots[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
 #pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      float x[8], f8[8], p8[8];
-      lds8(F + (c0 + g * 8) * 4, f8);
-      lds8(P + (c0 + g * 8) * 4, p8);
+  for (int j = 0; j < 32; ++j) {
+    const int c = frag_col(t, j, 0);
+    float f2[2], p2[2];
+    asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(f2[0]), "=f"(f2[1]) : "r"(F + c * 4));
+    asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(p2[0]), "=f"(p2[1]) : "r"(P + c * 4));
+    float v[4] = {d[4 * j], d[4 * j + 1], d[4 * j + 2], d[4 * j + 3]};
+    if (kStash) {
+      const float4 q = stash_load4(stash, 4 * j);
+      v[0] = q.x; v[1] = q.y; v[2] = q.z; v[3] = q.w;
+    }
 #pragma unroll
-      for (int j = 0; j < 8; j += 2) {
-        const float2 s2 = sin_reduced2(__ffma2_rn(make_float2(f8[j], f8[j + 1]),
-                                                  make_float2(__uint_as_float(raw[g * 8 + j]), __uint_as_float(raw[g * 8 + j + 1])),
-                                                  make_float2(p8[j], p8[j + 1])));
-        x[j] = s2.x;
-        x[j + 1] = s2.y;
-      }
-      if (kHead == 1) {
-        float w8[8];
-        lds8(wsig + (c0 + g * 8) * 4, w8);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) d0 = fmaf(x[j], w8[j], d0);
-      }
+    for (int i = 0; i < 2; ++i) {
+      const float2 x = sin_reduced2(ffma2(make_float2(f2[0], f2[1]), make_float2(v[2 * i], v[2 * i + 1]),
+                                          make_float2(p2[0], p2[1])));
+      if (kHead == 1) dots[i][0] = fmaf(x.y, m.w_sigma[c + 1], fmaf(x.x, m.w_sigma[c], dots[i][0]));
       if (kHead == 2) {
-        float w0[8], w1[8], w2[8];
-        lds8(wrgb + (c0 + g * 8) * 4, w0);
-        lds8(wrgb + (kRH + c0 + g * 8) * 4, w1);
-        lds8(wrgb + (2 * kRH + c0 + g * 8) * 4, w2);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          d0 = fmaf(x[j], w0[j], d0);
-          d1 = fmaf(x[j], w1[j], d1);
-          d2 = fmaf(x[j], w2[j], d2);
-        }
+        for (int h = 0; h < 3; ++h) dots[i][h] = fmaf(x.y, m.w_rgb[h * kRH + c + 1], fmaf(x.x, m.w_rgb[h * kRH + c], dots[i][h]));
       }
-      store_a8<kPasses == 3>(m.a_hi + kc * kRA, m.a_lo + kc * kRA, row, h * 32 + g * 8, x);
-    }
-    if (!defer_arrive) {
-      tc_fence_before();
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(m.bars + RA_FULL + kc);
+      const int kc = c >> 6;
+      store_a2<kPasses == 3>(m.a_hi + kc * kRA, m.a_lo + kc * kRA, g * 64 + frag_row(t, i), c & 63, x.x, x.y);
     }
   }
-  if (defer_arrive) {
-    tc_fence_before();
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0)
-      for (int kc = 0; kc < 4; ++kc) mbar_arrive(m.bars + RA_FULL + kc);
+  if (kHead != 0) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+#pragma unroll
+      for (int h = 0; h < 3; ++h) {
+        if (kHead == 1 && h > 0) break;
+        float v = dots[i][h];
+        v += __shfl_xor_sync(0xffffffffu, v, 1);
+        v += __shfl_xor_sync(0xffffffffu, v, 2);
+        if ((t & 3) == 0) m.part[(g * 64 + frag_row(t, i)) * 4 + (kHead == 1 ? 0 : 1 + h)] = v;
+      }
+    }
   }
-  if (kHead == 1) m.part[(h * 128 + row) * 4 + 0] = d0;
-  if (kHead == 2) {
-    m.part[(h * 128 + row) * 4 + 1] = d0;
-    m.part[(h * 128 + row) * 4 + 2] = d1;
-    m.part[(h * 128 + row) * 4 + 3] = d2;
-  }
+  fence_proxy_async_smem();
+  named_barrier(2 + g, 128);
 }
 
 template <int kPasses>
@@ -239,20 +204,13 @@ __global__ void __launch_bounds__(kRenThreads, 1) render_mlp_kernel(RenderArgs a
   }
   for (int i = threadIdx.x; i < 3 * kRH; i += blockDim.x) m.w_rgb[i] = a.w_rgb[i];
   if (threadIdx.x == 0) {
-    for (int i = 0; i < 4; ++i) mbar_init(m.bars + RA_FULL + i, 8);
     for (int i = 0; i < kRenStages; ++i) {
       mbar_init(m.bars + RB_FULL + i, 1);
-      mbar_init(m.bars + RB_EMPTY + i, 1);
+      mbar_init(m.bars + RB_EMPTY + i, 2);     // one arrival per warpgroup
     }
-    mbar_init(m.bars + RL_FULL, 1);
     fence_mbar_init();
   }
-  if (warp == 8) tmem_alloc<512>(m.tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *m.tmem_slot;
-  const uint32_t accA = tmem, accB = tmem + 256;
 
   const int S = a.S;
   const int rpt = 128 / S;                               // rays per tile
@@ -262,32 +220,64 @@ __global__ void __launch_bounds__(kRenThreads, 1) render_mlp_kernel(RenderArgs a
   const long N = static_cast<long>(a.R) * S;
 
   if (warp < 8) {
-    const int q = warp & 3, h = warp >> 2;
-    const int row = q * 32 + lane;
-    const int rl = row / S, s = row % S;                 // ray within the tile, sample along the ray
-    uint32_t lph = 0;                                    // RL_FULL phase
+    regs_inc<kMmaRegs>();
+    const int g = warp >> 2, t = threadIdx.x & 127;
+    const int tid = threadIdx.x;                         // 0..255: per-point scalar work uses point row = tid (< 128)
+    float d[128];
+    __align__(16) float stash[128];
+    uint32_t st = 0, ph = 0;
+    // one weight stage: wait, issue on this warpgroup's 64 rows, release the previous stage once its wgmmas are done
+    uint32_t prev = ~0u;
+    auto stage = [&](uint32_t a_tile, uint32_t a_tile2, bool two, bool accumulate) {
+      mbar_wait(m.bars + RB_FULL + st, ph);
+      acc_fence(d);
+      wgmma_fence();
+      const uint32_t bt = smem_u32(m.b_st + st * kRB);
+      wg_k64<256>(d, a_tile, bt, accumulate);
+      if (two) wg_k64<256>(d, a_tile2, bt, true);
+      wgmma_commit();
+      wgmma_wait<1>();
+      acc_fence(d);
+      if (prev != ~0u && t == 0) mbar_arrive(m.bars + RB_EMPTY + prev);
+      prev = st;
+      if (++st == kRenStages) { st = 0; ph ^= 1; }
+    };
+    // one GEMM of K = 64 * nk over operand chunks k0.. into the accumulator
+    auto layer = [&](int k0, int nk, bool accumulate) {
+      for (int kc = k0; kc < k0 + nk; ++kc) {
+        const uint32_t ahi = smem_u32(m.a_hi + kc * kRA) + g * 64 * 128, alo = smem_u32(m.a_lo + kc * kRA) + g * 64 * 128;
+        stage(ahi, alo, kPasses == 3, accumulate || kc > k0);
+        if (kPasses == 3) stage(ahi, ahi, false, true);
+      }
+      wgmma_wait<0>();
+      acc_fence(d);
+      if (t == 0) mbar_arrive(m.bars + RB_EMPTY + prev);
+      prev = ~0u;
+    };
     int cur_b = -1;
     for (int it = 0; it < my_tiles; ++it) {
       const int tile = blockIdx.x + it * gridDim.x;
       const int b = tile / tiles_per_img;
       const int ray0 = (tile % tiles_per_img) * rpt;
-      const int ray = ray0 + rl;
-      const bool valid = ray < a.R;
-      const long gp = static_cast<long>(b) * N + static_cast<long>(ray) * S + s;
       if (b != cur_b) {
         ren_rows_barrier();
-        for (int i = threadIdx.x; i < kFilmLayers * 2 * kRH; i += 256)
+        for (int i = tid; i < kFilmLayers * 2 * kRH; i += 256)
           m.film[i] = a.film[static_cast<long>(b) * kFilmLayers * 2 * kRH + i];
         cur_b = b;
         ren_rows_barrier();
       }
-      // ---- A0: point record -> operand chunk 0 (K = 64: 36 values + zeros)
+      // ---- A0: point record -> operand chunk 0 (K = 64: 36 values + zeros); thread t: row 64g + t/2, k half t&1
       {
+        const int row = g * 64 + (t >> 1), kh = t & 1;
+        const int rl = row / S, s = row % S;
+        const int ray = ray0 + rl;
+        const bool valid = ray < a.R;
+        const long gp = static_cast<long>(b) * N + static_cast<long>(ray) * S + s;
         float x[8];
         const float4* rp = reinterpret_cast<const float4*>(a.rec + gp * 36);
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const int k0 = h * 32 + g * 8;
+        for (int gi = 0; gi < 4; ++gi) {
+          const int k0 = kh * 32 + gi * 8;
 #pragma unroll
           for (int u = 0; u < 2; ++u) {
             const int f4 = (k0 >> 2) + u;
@@ -297,57 +287,66 @@ __global__ void __launch_bounds__(kRenThreads, 1) render_mlp_kernel(RenderArgs a
           }
           store_a8<kPasses == 3>(m.a_hi, m.a_lo, row, k0, x);
         }
-        if (h == 0) m.zs[row] = (valid && a.z_vals) ? a.z_vals[gp] : 0.f;
+        if (kh == 0) m.zs[row] = (valid && a.z_vals) ? a.z_vals[gp] : 0.f;
         fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(m.bars + RA_FULL + 0);
+        named_barrier(2 + g, 128);
       }
-      // ---- E0 .. E6
-      mbar_wait_sleep(m.bars + RL_FULL, lph); lph ^= 1; tc_fence_after();
-      film_epilogue<kPasses, 0>(m, accA, 0, warp, lane, /*defer=*/true);
-      mbar_wait_sleep(m.bars + RL_FULL, lph); lph ^= 1; tc_fence_after();
-      film_epilogue<kPasses, 0>(m, accB, 1, warp, lane, false);
-      mbar_wait_sleep(m.bars + RL_FULL, lph); lph ^= 1; tc_fence_after();
-      film_epilogue<kPasses, 0>(m, accA, 2, warp, lane, false);
-      mbar_wait_sleep(m.bars + RL_FULL, lph); lph ^= 1; tc_fence_after();
-      film_epilogue<kPasses, 0>(m, accB, 3, warp, lane, false);
-      mbar_wait_sleep(m.bars + RL_FULL, lph); lph ^= 1; tc_fence_after();
-      film_epilogue<kPasses, 0>(m, accA, 4, warp, lane, false);
-      mbar_wait_sleep(m.bars + RL_FULL, lph); lph ^= 1; tc_fence_after();
-      film_epilogue<kPasses, 1>(m, accB, 5, warp, lane, false);
-      mbar_wait_sleep(m.bars + RL_FULL, lph); lph ^= 1; tc_fence_after();
-      film_epilogue<kPasses, 2>(m, accA, 6, warp, lane, false);
+      // ---- MLP
+      layer(0, 1, false);                                   // L0c
+      stash_store(stash, d);
+      layer(0, 1, false);                                   // L0g
+      film_epilogue<kPasses, 0>(m, d, stash, 1, g, t);      // E1
+      layer(0, 4, false);                                   // L1b
+      film_epilogue<kPasses, 0, true>(m, d, stash, 0, g, t);  // E0 (coord pre-activation from the stash)
+      layer(0, 4, true);                                    // L1a, accumulating onto L1b
+      film_epilogue<kPasses, 0>(m, d, stash, 2, g, t);      // E2
+      layer(0, 4, false);                                   // network.1
+      film_epilogue<kPasses, 0>(m, d, stash, 3, g, t);      // E3
+      layer(0, 4, false);                                   // network.2
+      film_epilogue<kPasses, 0>(m, d, stash, 4, g, t);      // E4
+      layer(0, 4, false);                                   // network.3
+      film_epilogue<kPasses, 1>(m, d, stash, 5, g, t);      // E5 + sigma head
+      layer(0, 4, false);                                   // color
+      film_epilogue<kPasses, 2>(m, d, stash, 6, g, t);      // E6 + rgb heads
+      layer(0, 4, false);                                   // feature
 
+      ren_rows_barrier();                                   // heads of both warpgroups in part[], operands no longer read
       if (a.raw_out) {
         // ---- per-point outputs of COORDCONCATSIREN.forward (modulated.py:70-73): [rgb, feat, sigma]
-        ren_rows_barrier();
-        float* po = a.raw_out + gp * kRayOut;
-        if (h == 0 && valid) {
-          po[259] = m.part[row * 4] + m.part[(128 + row) * 4] + a.heads_b[0];
-          for (int j = 0; j < 3; ++j) {
-            const float dot = m.part[row * 4 + 1 + j] + m.part[(128 + row) * 4 + 1 + j] + a.heads_b[1 + j];
-            po[j] = 1.f / (1.f + expf(-dot));
+        if (tid < 128) {
+          const int row = tid, rl = row / S, s = row % S, ray = ray0 + rl;
+          const long gp = static_cast<long>(b) * N + static_cast<long>(ray) * S + s;
+          if (ray < a.R) {
+            float* po = a.raw_out + gp * kRayOut;
+            po[259] = m.part[row * 4] + a.heads_b[0];
+            for (int j = 0; j < 3; ++j) {
+              const float dot = m.part[row * 4 + 1 + j] + a.heads_b[1 + j];
+              po[j] = 1.f / (1.f + expf(-dot));
+            }
           }
         }
-        mbar_wait_sleep(m.bars + RL_FULL, lph); lph ^= 1; tc_fence_after();
-#pragma unroll 1
-        for (int kc = 0; kc < 4; ++kc) {
-          const int c0 = kc * 64 + h * 32;
-          uint32_t raw[32];
-          tmem_ld32(accB + (static_cast<uint32_t>(q * 32) << 16) + c0, raw);
-          tmem_ld_wait();
-          if (valid)
-            for (int j = 0; j < 32; ++j) po[3 + c0 + j] = __uint_as_float(raw[j]) + m.b_feat[c0 + j];
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int row = g * 64 + frag_row(t, i), rl = row / S, s = row % S, ray = ray0 + rl;
+          if (ray >= a.R) continue;
+          float* po = a.raw_out + (static_cast<long>(b) * N + static_cast<long>(ray) * S + s) * kRayOut + 3;
+#pragma unroll
+          for (int j = 0; j < 32; ++j) {
+            const int c = frag_col(t, j, 0);
+            po[c] = d[4 * j + 2 * i] + m.b_feat[c];
+            po[c + 1] = d[4 * j + 2 * i + 1] + m.b_feat[c + 1];
+          }
         }
-        tc_fence_before();
         ren_rows_barrier();
         continue;
       }
-      // ---- compositing weights (volume_rendering.py:12-38); overlaps the feature GEMM
-      ren_rows_barrier();
+      // ---- compositing weights (volume_rendering.py:12-38)
       float alpha = 0.f;
-      if (h == 0) {
-        const float sigma = m.part[row * 4] + m.part[(128 + row) * 4] + a.heads_b[0];
+      if (tid < 128) {
+        const int row = tid, rl = row / S, s = row % S, ray = ray0 + rl;
+        const long gp = static_cast<long>(b) * N + static_cast<long>(ray) * S + s;
+        const bool valid = ray < a.R;
+        const float sigma = m.part[row * 4] + a.heads_b[0];
         const float delta = (s == S - 1) ? 1e9f : m.zs[row + 1] - m.zs[row];
         float pre = sigma;
         if (a.noise) pre += (valid ? a.noise[gp] : 0.f) * a.noise_std;
@@ -356,154 +355,86 @@ __global__ void __launch_bounds__(kRenThreads, 1) render_mlp_kernel(RenderArgs a
         m.tr[row] = 1.f - alpha + 1e-12f;
       }
       ren_rows_barrier();
-      if (h == 0) {
+      if (tid < 128) {
+        const int row = tid, rl = row / S, s = row % S;
         float T = 1.f;
         for (int k = 0; k < s; ++k) T *= m.tr[rl * S + k];
-        m.wgt[row] = valid ? alpha * T : 0.f;
+        m.wgt[row] = ray0 + rl < a.R ? alpha * T : 0.f;
       }
       ren_rows_barrier();
-      if (h == 0 && s == 0) {
+      if (tid < rpt) {
         float W = 0.f;
-        for (int k = 0; k < S; ++k) W += m.wgt[rl * S + k];
-        m.rayw[rl] = W;
+        for (int k = 0; k < S; ++k) W += m.wgt[tid * S + k];
+        m.rayw[tid] = W;
       }
       ren_rows_barrier();
-      const float Wsum = m.rayw[rl];
-      float w = m.wgt[row];
-      const float w_depth = w + ((s == S - 1) ? 1.f - Wsum : 0.f);
-      if (a.last_back) w = w_depth;
-      if (a.weights_out && h == 0 && valid) a.weights_out[gp] = w;
-      const float back = a.white_back ? 1.f - Wsum : 0.f;
+      if (tid < 128) {
+        const int row = tid, rl = row / S, s = row % S, ray = ray0 + rl;
+        const float Wsum = m.rayw[rl];
+        float w = m.wgt[row];
+        const float w_depth = w + ((s == S - 1) ? 1.f - Wsum : 0.f);
+        if (a.last_back) w = w_depth;
+        if (a.weights_out && ray < a.R) a.weights_out[static_cast<long>(b) * N + static_cast<long>(ray) * S + s] = w;
+        m.tr[row] = w;                                     // the weight actually applied (tr is free again)
+        m.wgt[row] = w_depth;
+      }
+      ren_rows_barrier();
 
-      // ---- E7: feature accumulator -> weighted sum over the ray
-      mbar_wait_sleep(m.bars + RL_FULL, lph); lph ^= 1; tc_fence_after();
-      float* ro = a.ray_out + (static_cast<long>(b) * a.R + ray) * kRayOut;
-      if (S == 32) {
-        // one warp == one ray: shuffle transpose-reduce, lane j ends with column j's sum
-#pragma unroll 1
-        for (int kc = 0; kc < 4; ++kc) {
-          const int c0 = kc * 64 + h * 32;
-          uint32_t raw[32];
-          tmem_ld32(accB + (static_cast<uint32_t>(q * 32) << 16) + c0, raw);
-          tmem_ld_wait();
-          float v[32];
+      // ---- E7: weighted feature sum over each ray, 64 columns at a time through a [128 x 65] scratch (operand buffer)
+      float* scratch = reinterpret_cast<float*>(m.a_hi);
+      const float wr[2] = {m.tr[g * 64 + frag_row(t, 0)], m.tr[g * 64 + frag_row(t, 1)]};
 #pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            float b8[8];
-            uint32_t bfa = smem_u32(m.b_feat);
-            opaque(bfa);
-            lds8(bfa + (c0 + g * 8) * 4, b8);
+      for (int cg = 0; cg < 4; ++cg) {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) v[g * 8 + j] = w * (__uint_as_float(raw[g * 8 + j]) + b8[j]);
+        for (int i = 0; i < 2; ++i) {
+          const int row = g * 64 + frag_row(t, i);
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const int j = cg * 8 + jj, c = frag_col(t, j, 0);
+            scratch[row * kScr + (c & 63)] = wr[i] * (d[4 * j + 2 * i] + m.b_feat[c]);
+            scratch[row * kScr + (c & 63) + 1] = wr[i] * (d[4 * j + 2 * i + 1] + m.b_feat[c + 1]);
           }
-          const float tot = transpose_reduce32r(v, lane);
-          if (valid) ro[c0 + lane] = tot + back;   // `ro`/`valid` are warp-uniform here (S == 32)
-        }
-        if (h == 0) {
-          float e[4];
-#pragma unroll
-          for (int j = 0; j < 3; ++j) {
-            const float dot = m.part[row * 4 + 1 + j] + m.part[(128 + row) * 4 + 1 + j] + a.heads_b[1 + j];
-            e[j] = w / (1.f + expf(-dot));
-          }
-          e[3] = w_depth * m.zs[row];
-#pragma unroll
-          for (int j = 0; j < 4; ++j)
-            for (int o = 16; o > 0; o >>= 1) e[j] += __shfl_xor_sync(0xffffffffu, e[j], o);
-          if (valid && lane < 4) ro[256 + lane] = (lane == 0 ? e[0] : lane == 1 ? e[1] : lane == 2 ? e[2] : e[3]) + (lane < 3 ? back : 0.f);
-        }
-        tc_fence_before();
-      } else {
-        // generic S: stage w*feat through shared memory (aliases the operand buffer, free by now)
-        float* scratch = reinterpret_cast<float*>(m.a_hi);          // [2][128][33]
-        float* mine = scratch + (h * 128 + row) * 33;
-#pragma unroll 1
-        for (int kc = 0; kc < 4; ++kc) {
-          const int c0 = kc * 64 + h * 32;
-          uint32_t raw[32];
-          tmem_ld32(accB + (static_cast<uint32_t>(q * 32) << 16) + c0, raw);
-          tmem_ld_wait();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) mine[j] = w * (__uint_as_float(raw[j]) + m.b_feat[c0 + j]);
-          ren_rows_barrier();
-          // 256 threads: (ray r2, column j2) pairs; thread handles rays r2, r2 + 8, ...
-          for (int r2 = warp & 3; r2 < rpt; r2 += 4) {
-            float acc = 0.f;
-            const float* src = scratch + (h * 128 + r2 * S) * 33 + lane;
-            for (int k = 0; k < S; ++k) acc += src[k * 33];
-            if (ray0 + r2 < a.R)
-              a.ray_out[(static_cast<long>(b) * a.R + ray0 + r2) * kRayOut + c0 + lane] =
-                  acc + (a.white_back ? 1.f - m.rayw[r2] : 0.f);
-          }
-          ren_rows_barrier();
-        }
-        if (h == 0) {
-          float e[4];
-#pragma unroll
-          for (int j = 0; j < 3; ++j) {
-            const float dot = m.part[row * 4 + 1 + j] + m.part[(128 + row) * 4 + 1 + j] + a.heads_b[1 + j];
-            e[j] = w / (1.f + expf(-dot));
-          }
-          e[3] = w_depth * m.zs[row];
-#pragma unroll
-          for (int j = 0; j < 4; ++j) mine[j] = e[j];
         }
         ren_rows_barrier();
-        if (h == 0 && s == 0 && valid) {
-          float e[4] = {0.f, 0.f, 0.f, 0.f};
-          for (int k = 0; k < S; ++k)
-#pragma unroll
-            for (int j = 0; j < 4; ++j) e[j] += scratch[(rl * S + k) * 33 + j];
-          ro[256] = e[0] + back; ro[257] = e[1] + back; ro[258] = e[2] + back; ro[259] = e[3];
-        }
-        tc_fence_before();
-        ren_rows_barrier();   // scratch is the next tile's operand buffer
-      }
-    }
-  } else if (warp == 8) {
-    {      // the warp walks the loops, one elected lane issues (umma.cuh: elect_one_sync)
-      const bool leader = elect_one_sync();
-      const uint32_t idesc = umma_idesc_bf16(128, 256);
-      uint32_t st = 0, ph = 0;
-      uint32_t aph[4] = {0, 0, 0, 0};
-      auto wait_a = [&](int kc) {
-        mbar_wait(m.bars + RA_FULL + kc, aph[kc]);
-        aph[kc] ^= 1;
-        tc_fence_after();
-      };
-      auto A_hi = [&](int kc) { return smem_u32(m.a_hi + kc * kRA); };
-      auto A_lo = [&](int kc) { return smem_u32(m.a_lo + kc * kRA); };
-      for (int it = 0; it < my_tiles; ++it) {
-        // L0: coord -> A, geo -> B (both read operand chunk 0)
-        wait_a(0);
-        ren_mma_chunk<kPasses>(m, leader, st, ph, accA, A_hi(0), A_lo(0), idesc, false);
-        ren_mma_chunk<kPasses>(m, leader, st, ph, accB, A_hi(0), A_lo(0), idesc, false);
-        umma_commit_if(leader, m.bars + RL_FULL);
-        // L1a: a x Wn0[:, :256] -> A
-        for (int kc = 0; kc < 4; ++kc) {
-          wait_a(kc);
-          ren_mma_chunk<kPasses>(m, leader, st, ph, accA, A_hi(kc), A_lo(kc), idesc, kc > 0);
-        }
-        umma_commit_if(leader, m.bars + RL_FULL);
-        // L1b: g x Wn0[:, 256:] -> A (accumulate)
-        for (int kc = 0; kc < 4; ++kc) {
-          wait_a(kc);
-          ren_mma_chunk<kPasses>(m, leader, st, ph, accA, A_hi(kc), A_lo(kc), idesc, true);
-        }
-        umma_commit_if(leader, m.bars + RL_FULL);
-        // network.1, .2, .3, color, feature: B, A, B, A, B
-        for (int l = 0; l < 5; ++l) {
-          const uint32_t acc = (l & 1) ? accA : accB;
-          for (int kc = 0; kc < 4; ++kc) {
-            wait_a(kc);
-            ren_mma_chunk<kPasses>(m, leader, st, ph, acc, A_hi(kc), A_lo(kc), idesc, kc > 0);
+        {
+          const int col = tid & 63;
+          for (int r2 = tid >> 6; r2 < rpt; r2 += 4) {
+            float acc = 0.f;
+            const float* src = scratch + (r2 * S) * kScr + col;
+            for (int k = 0; k < S; ++k) acc += src[k * kScr];
+            if (ray0 + r2 < a.R)
+              a.ray_out[(static_cast<long>(b) * a.R + ray0 + r2) * kRayOut + cg * 64 + col] =
+                  acc + (a.white_back ? 1.f - m.rayw[r2] : 0.f);
           }
-          umma_commit_if(leader, m.bars + RL_FULL);
         }
+        ren_rows_barrier();
       }
+      // rgb and depth: per point into the scratch, then one thread per ray
+      if (tid < 128) {
+        const int row = tid;
+        const float w = m.tr[row];
+#pragma unroll
+        for (int j = 0; j < 3; ++j) {
+          const float dot = m.part[row * 4 + 1 + j] + a.heads_b[1 + j];
+          scratch[row * kScr + j] = w / (1.f + expf(-dot));
+        }
+        scratch[row * kScr + 3] = m.wgt[row] * m.zs[row];
+      }
+      ren_rows_barrier();
+      if (tid < rpt && ray0 + tid < a.R) {
+        float e[4] = {0.f, 0.f, 0.f, 0.f};
+        for (int k = 0; k < S; ++k)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) e[j] += scratch[(tid * S + k) * kScr + j];
+        const float back = a.white_back ? 1.f - m.rayw[tid] : 0.f;
+        float* ro = a.ray_out + (static_cast<long>(b) * a.R + ray0 + tid) * kRayOut;
+        ro[256] = e[0] + back; ro[257] = e[1] + back; ro[258] = e[2] + back; ro[259] = e[3];
+      }
+      ren_rows_barrier();   // scratch is the next tile's operand buffer
     }
   } else {
-    if (lane == 0) {
+    regs_dec<kProducerRegs>();
+    if (warp == 8 && lane == 0) {
       uint32_t st = 0, ph = 0;
       for (int it = 0; it < my_tiles; ++it)
         for (int sidx = 0; sidx < kWeightStages; ++sidx) {
@@ -515,9 +446,6 @@ __global__ void __launch_bounds__(kRenThreads, 1) render_mlp_kernel(RenderArgs a
         }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 8) tmem_dealloc<512>(tmem);
 }
 
 }  // namespace hg

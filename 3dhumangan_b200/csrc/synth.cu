@@ -7,21 +7,11 @@
 // tiles of 128 consecutive pixels): the 128 KB a CTA reads / writes per tile are CONTIGUOUS, and every
 // 32-channel slice of a tile is one contiguous 16 KB block (one cp.async.bulk).
 //
-// Per CTA (512 threads), persistent over tiles of 128 pixels of one image:
-//   warps 0-7   operand team: build the bf16 hi/lo A operand of the NEXT tile in a 2-slot ring of
-//               [128 x 64] K-major SW128 chunks (BN scale/shift, SPADE modulation, LeakyReLU fused)
-//   warps 8-11  epilogue team: drain the fp32 accumulator of the PREVIOUS tile from TMEM (warp 8+q owns lanes
-//               32q..32q+31, all 256 columns): bias, residual, ToRGB, per-channel sum / sum-of-squares for the
-//               next BatchNorm (so SyncBN statistics never need their own pass), plane stores
-//   warp 12     MMA issuer: the warp walks the tile / chunk loops in convergent code, its elected lane issues tcgen05.mma
-//               (M=128, N=256, K=16; bf16x3 split or plain bf16)
-//   warp 13     one thread streams the packed weight tiles from L2 (cp.async.bulk, 2 x 32 KB stages)
-//   warp 14     one thread streams activation slices (ring slots 0-2, operand team) from HBM with cp.async.bulk
-//   warp 15     one thread streams residual slices (ring slots 3-4, epilogue team).  Two threads, not one: with a
-//               single producer the two rings are coupled by program order, and in the pixel-style variant
-//               (gamma/beta GEMM of tile t+1 waits for the epilogue of tile t) that coupling deadlocks.
-// The two TMEM halves (2 x 256 columns) alternate between tiles, so the epilogue of tile t, the MMAs of tile
-// t+1 and the operand production of tile t+1/t+2 overlap.
+// Per CTA (384 threads), persistent over tiles of 128 pixels of one image: warpgroup g (warps 4g..4g+3) builds the bf16
+// hi/lo operand rows of pixels 64g..64g+63 (BN, SPADE modulation, LeakyReLU fused), issues their wgmmas ([64 x 256] fp32
+// accumulator in registers) and runs the epilogue (bias, residual, ToRGB, next-BatchNorm statistics, plane stores); warps
+// 8, 9, 10 each stream one ring with cp.async.bulk (weights, activation slices, residual slices: one producer per ring,
+// since a single producer couples the rings by program order and deadlocks).
 //
 // Two variants:
 //   const-style : gamma/beta are per-sample vectors (blocks whose style map is spatially constant, 12 of 18
@@ -29,9 +19,7 @@
 //   pixel-style : gamma/beta come from a second GEMM on relu(bilinear_up(P_lr)) where
 //                 P_lr = W_shared . feature_maps + b at RENDER resolution (W_shared commutes with the bilinear
 //                 up-sample), so the 28x larger up-sampled style map of map3d_generator.py:244-245 is never
-//                 materialised.  TMEM plan per tile t (R = half t&1, R' = the other, still being drained):
-//                 G1(gamma|beta, channels 0-127) -> R, G1(channels 128-255) -> R' once the epilogue of t-1 is
-//                 done, y chunks 0,1 <- R, conv accumulator -> R, y chunks 2,3 <- R'.
+//                 materialised.  Per conv K chunk the [gamma | beta] GEMM of its 64 channels runs first (N = 128).
 //
 // The const-style kernel doubles as the library's blocked 1x1-convolution engine (runtime fields at the end of SpadeArgs):
 // K of 64..512 input channels from one or two sources, LeakyReLU / sine / identity operand transform, and -- template
@@ -41,16 +29,14 @@
 // per-(sample, channel) sums the BatchNorm / FiLM gradients need (DESIGN.md "Backward").
 //
 // Ring protocol note: every consumer warp of a staging ring waits for and releases EVERY slice in order
-// (only the owning column half reads it).  With per-half arrivals a slot of an odd-sized ring alternates
-// between halves, a fast half gets two phases ahead and the parity wait succeeds on a stale phase -- that race
-// produced launch failures in an earlier version (DESIGN.md "Pitfalls").
+// (see ring_take / ring_release).
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hg {
 
 constexpr int kC = 256;             // channels (hidden_dim == feature_dim == 256)
-constexpr int kSynThreads = 512;
+constexpr int kSynThreads = 384;
 constexpr int kSynStages = 2;       // weight stages
 constexpr int kASlots = 2;          // operand ring
 constexpr int kXSlots = 5;          // staging slots in total
@@ -98,10 +84,11 @@ struct SpadeArgs {
 };
 
 struct SynSmem {
-  uint8_t* a_hi;   // [kASlots] chunks
+  uint8_t* a_hi;   // operand chunks: const-style a 2-slot ring; pixel-style A1 (2 chunks) + one y chunk
   uint8_t* a_lo;
   uint8_t* b_st;
-  float* x_st;     // [kXSlots][32][128]
+  float* x_st;     // staging slots [32][128]: activation ring, then residual ring
+  int xs_n, ss_n;  // slots of the two rings
   float* tab_g1;   // [C]  (const: g1 | pixel: bn scale)
   float* tab_g0;   // [C]  (const: g0 | pixel: bn shift)
   float* tab_bias; // [C]
@@ -111,17 +98,21 @@ struct SynSmem {
   float* st_sum;   // [C]
   float* st_sq;    // [C]
   uint64_t* bars;
-  uint32_t* tmem_slot;
 };
 
+// const-style: 2 operand slots, 3 + 2 staging slots; pixel-style: 3 operand chunks, 2 + 1 staging slots
+template <bool kPixel>
 __device__ __forceinline__ SynSmem carve(uint8_t* raw) {
+  constexpr int kA = kPixel ? 3 : kASlots, kX = kPixel ? 3 : kXSlots;
   uint8_t* s = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~uintptr_t(1023));
   SynSmem m;
   m.a_hi = s;
-  m.a_lo = s + kASlots * kAChunk;
-  m.b_st = s + 2 * kASlots * kAChunk;
+  m.a_lo = s + kA * kAChunk;
+  m.b_st = s + 2 * kA * kAChunk;
   m.x_st = reinterpret_cast<float*>(m.b_st + kSynStages * kBStage);
-  float* f = m.x_st + kXSlots * (kXSlice / 4);
+  m.xs_n = kPixel ? 2 : kXs;
+  m.ss_n = kPixel ? 1 : kSs;
+  float* f = m.x_st + kX * (kXSlice / 4);
   m.tab_g1 = f; f += kC;
   m.tab_g0 = f; f += kC;
   m.tab_bias = f; f += kC;
@@ -131,18 +122,17 @@ __device__ __forceinline__ SynSmem carve(uint8_t* raw) {
   m.st_sum = f; f += kC;
   m.st_sq = f; f += kC;
   m.bars = reinterpret_cast<uint64_t*>(f);
-  m.tmem_slot = reinterpret_cast<uint32_t*>(m.bars + 40);
   return m;
 }
 constexpr uint32_t kSynSmemBytes = 2 * kASlots * kAChunk + kSynStages * kBStage + kXSlots * kXSlice +
-                                   (kC * 9 + 512) * 4 + 40 * 8 + 16 + 1024;
-static_assert(kSynSmemBytes <= 232448, "shared memory budget");
+                                   (kC * 9 + 512) * 4 + 24 * 8 + 1024;
+constexpr uint32_t kPixSmemBytes = 2 * 3 * kAChunk + kSynStages * kBStage + 3 * kXSlice + (kC * 9 + 512) * 4 + 24 * 8 + 1024;
+static_assert(kSynSmemBytes <= 232448 && kPixSmemBytes <= 232448, "shared memory budget");
 
 // barrier slots
-enum { A_FULL = 0 /*2*/, A_EMPTY = 2 /*2*/, B_FULL = 4 /*2*/, B_EMPTY = 6 /*2*/, ACC_FULL = 8 /*2*/,
-       ACC_EMPTY = 10 /*2*/, G1A_FULL = 12, G1B_FULL = 13, A1_FULL = 14, X_FULL = 16 /*5*/, X_EMPTY = 24 /*5*/ };
+enum { B_FULL = 0 /*2*/, B_EMPTY = 2 /*2*/, X_FULL = 4 /*5*/, X_EMPTY = 12 /*5*/ };
 
-__device__ __forceinline__ void rows_barrier() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+__device__ __forceinline__ void rows_barrier() { named_barrier(1, 256); }
 
 __device__ __forceinline__ float lrelu02(float v) { return v > 0.f ? v : 0.2f * v; }
 
@@ -156,30 +146,15 @@ __device__ __forceinline__ float reduce_2pi(float t) {
 }
 __device__ __forceinline__ float sin_red(float t) { return __sinf(reduce_2pi(t)); }
 __device__ __forceinline__ float cos_red(float t) { return __cosf(reduce_2pi(t)); }
-// the same reduction on a pair (packed fp32: identical operations per lane)
+// the same reduction on a pair (identical operations per lane)
 __device__ __forceinline__ float2 reduce_2pi2(float2 t) {
-  const float2 y = __fmul2_rn(t, make_float2(0.15915494309189535f, 0.15915494309189535f));
-  const float2 k = __fadd2_rn(__fadd2_rn(y, make_float2(12582912.f, 12582912.f)), make_float2(-12582912.f, -12582912.f));
-  const float2 r = __ffma2_rn(k, make_float2(-6.2831854820251465f, -6.2831854820251465f), t);
-  return __ffma2_rn(k, make_float2(1.7484555314695172e-07f, 1.7484555314695172e-07f), r);
+  const float2 y = fmul2(t, make_float2(0.15915494309189535f, 0.15915494309189535f));
+  const float2 k = fadd2(fadd2(y, make_float2(12582912.f, 12582912.f)), make_float2(-12582912.f, -12582912.f));
+  const float2 r = ffma2(k, make_float2(-6.2831854820251465f, -6.2831854820251465f), t);
+  return ffma2(k, make_float2(1.7484555314695172e-07f, 1.7484555314695172e-07f), r);
 }
 __device__ __forceinline__ float2 sin_red2(float2 t) { const float2 r = reduce_2pi2(t); return make_float2(__sinf(r.x), __sinf(r.y)); }
 __device__ __forceinline__ float2 cos_red2(float2 t) { const float2 r = reduce_2pi2(t); return make_float2(__cosf(r.x), __cosf(r.y)); }
-
-// 32 lanes x 32 values: after the call lane j holds sum over lanes of v[j].
-__device__ __forceinline__ float transpose_reduce32(float (&v)[32], int lane) {
-#pragma unroll
-  for (int w = 16; w >= 1; w >>= 1) {
-    const bool upper = (lane & w) != 0;
-#pragma unroll
-    for (int i = 0; i < w; ++i) {
-      const float send = upper ? v[i] : v[i + w];
-      const float keep = upper ? v[i + w] : v[i];
-      v[i] = keep + __shfl_xor_sync(0xffffffffu, send, w);
-    }
-  }
-  return v[0];
-}
 
 struct TileMap {
   int T, first, stride, count;
@@ -193,7 +168,7 @@ struct TileMap {
 // ------------------------------------------------------------------------------------------
 // common setup
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void init_common(const SpadeArgs& a, const SynSmem& m, int warp) {
+__device__ __forceinline__ void init_common(const SpadeArgs& a, const SynSmem& m) {
   for (int i = threadIdx.x; i < kC; i += blockDim.x) {
     m.tab_bias[i] = a.bias[i];
     m.st_sum[i] = 0.f;
@@ -202,78 +177,74 @@ __device__ __forceinline__ void init_common(const SpadeArgs& a, const SynSmem& m
   if (a.rgb_w)
     for (int i = threadIdx.x; i < 3 * kC; i += blockDim.x) m.tab_rgbw[i] = a.rgb_w[i];
   if (threadIdx.x == 0) {
-    for (int i = 0; i < kASlots; ++i) {
-      mbar_init(m.bars + A_FULL + i, 8);
-      mbar_init(m.bars + A_EMPTY + i, 1);
-    }
     for (int i = 0; i < kSynStages; ++i) {
       mbar_init(m.bars + B_FULL + i, 1);
-      mbar_init(m.bars + B_EMPTY + i, 1);
+      mbar_init(m.bars + B_EMPTY + i, 2);             // one arrival per warpgroup
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(m.bars + ACC_FULL + i, 1);
-      mbar_init(m.bars + ACC_EMPTY + i, 4);     // the 4 epilogue warps
-    }
-    mbar_init(m.bars + G1A_FULL, 1);
-    mbar_init(m.bars + G1B_FULL, 1);
-    mbar_init(m.bars + A1_FULL, 8);
-    for (int i = 0; i < kXSlots; ++i) {
+    for (int i = 0; i < m.xs_n + m.ss_n; ++i) {
       mbar_init(m.bars + X_FULL + i, 1);
-      mbar_init(m.bars + X_EMPTY + i, i < kXs ? 8 : 4);   // operand team: 8 warps, epilogue team: 4 warps
+      mbar_init(m.bars + X_EMPTY + i, 8);             // every warp of both warpgroups
     }
     fence_mbar_init();
   }
-  if (warp == 12) tmem_alloc<512>(m.tmem_slot);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
 }
 
 // ------------------------------------------------------------------------------------------
-// warp 13: weight stages.  Every tile consumes the same sequence: for each image `nstages` tiles of [256 x 64]
+// warp 8: weight stages.  Every tile consumes the same sequence: for each image `nstages` tiles of [256 x 64]
 // in storage order (kc-major, hi then lo); the lo tiles are skipped in 1-pass mode.
 // ------------------------------------------------------------------------------------------
 template <int kPasses>
-__device__ __forceinline__ void weight_producer_loop(const SynSmem& m, const uint8_t* const* imgs, const int* nstages,
-                                                     int nimgs, int num_my_tiles) {
+__device__ __forceinline__ void weight_producer_loop(const SynSmem& m, const uint8_t* img, int nstages, int num_my_tiles) {
   uint32_t st = 0, ph = 0;
   for (int t = 0; t < num_my_tiles; ++t)
-    for (int g = 0; g < nimgs; ++g)
-      for (int s = 0; s < nstages[g]; ++s) {
-        if (kPasses == 1 && (s & 1)) continue;
-        mbar_wait_backoff(m.bars + B_EMPTY + st, ph ^ 1);
-        mbar_arrive_expect_tx(m.bars + B_FULL + st, kBStage);
-        bulk_g2s(m.b_st + st * kBStage, imgs[g] + static_cast<size_t>(s) * kBStage, kBStage, m.bars + B_FULL + st);
-        if (++st == kSynStages) { st = 0; ph ^= 1; }
-      }
+    for (int s = 0; s < nstages; ++s) {
+      if (kPasses == 1 && (s & 1)) continue;
+      mbar_wait_backoff(m.bars + B_EMPTY + st, ph ^ 1);
+      mbar_arrive_expect_tx(m.bars + B_FULL + st, kBStage);
+      bulk_g2s(m.b_st + st * kBStage, img + static_cast<size_t>(s) * kBStage, kBStage, m.bars + B_FULL + st);
+      if (++st == kSynStages) { st = 0; ph ^= 1; }
+    }
 }
 
-struct MmaPipe {
-  uint32_t st = 0, ph = 0;
+// Weight-stage pipe of one warpgroup: wait for a stage, issue, and release the stage consumed one step earlier once its
+// wgmmas are done (both warpgroups release every stage).
+struct Pipe {
+  uint32_t st = 0, ph = 0, prev = ~0u;
 };
-
-// One K=64 chunk of a 3-pass (or 1-pass) product against the next weight stage(s).
-// `leader`: the elected lane of the (converged) MMA warp -- the whole warp walks the issue loops (umma.cuh: elect_one_sync).
-template <int kPasses>
-__device__ __forceinline__ void mma_chunk(const SynSmem& m, MmaPipe& p, bool leader, uint32_t tmem_d, uint32_t a_hi, uint32_t a_lo,
-                                          uint32_t idesc, bool accumulate) {
-  mbar_wait(m.bars + B_FULL + p.st, p.ph);
-  tc_fence_after();
-  umma_k64_if(leader, tmem_d, a_hi, smem_u32(m.b_st + p.st * kBStage), idesc, accumulate);
-  if (kPasses == 3) umma_k64_if(leader, tmem_d, a_lo, smem_u32(m.b_st + p.st * kBStage), idesc, true);
-  umma_commit_if(leader, m.bars + B_EMPTY + p.st);
-  if (++p.st == kSynStages) { p.st = 0; p.ph ^= 1; }
-  if (kPasses == 3) {
+template <int N, int kPasses>
+__device__ __forceinline__ void pipe_chunk(const SynSmem& m, Pipe& p, float (&d)[N / 2], uint32_t a_hi, uint32_t a_lo, bool accumulate,
+                                           int t) {
+#pragma unroll
+  for (int part = 0; part < (kPasses == 3 ? 2 : 1); ++part) {
     mbar_wait(m.bars + B_FULL + p.st, p.ph);
-    tc_fence_after();
-    umma_k64_if(leader, tmem_d, a_hi, smem_u32(m.b_st + p.st * kBStage), idesc, true);
-    umma_commit_if(leader, m.bars + B_EMPTY + p.st);
+    acc_fence(d);
+    wgmma_fence();
+    const uint32_t bt = smem_u32(m.b_st + p.st * kBStage);
+    if (part == 0) {
+      wg_k64<N>(d, a_hi, bt, accumulate);
+      if (kPasses == 3) wg_k64<N>(d, a_lo, bt, true);
+    } else {
+      wg_k64<N>(d, a_hi, bt, true);
+    }
+    wgmma_commit();
+    wgmma_wait<1>();
+    acc_fence(d);
+    if (p.prev != ~0u && t == 0) mbar_arrive(m.bars + B_EMPTY + p.prev);
+    p.prev = p.st;
     if (++p.st == kSynStages) { p.st = 0; p.ph ^= 1; }
   }
 }
+template <int N>
+__device__ __forceinline__ void pipe_drain(const SynSmem& m, Pipe& p, float (&d)[N / 2], int t) {
+  wgmma_wait<0>();
+  acc_fence(d);
+  if (p.prev != ~0u && t == 0) mbar_arrive(m.bars + B_EMPTY + p.prev);
+  p.prev = ~0u;
+}
 
 // ------------------------------------------------------------------------------------------
-// warp 14: activation slices (slots 0..2), warp 15: residual slices (slots 3..4): two independent rings.
+// warp 9: activation slices, warp 10: residual slices: two independent rings.
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ void ring_emit(const SynSmem& m, uint32_t& g, int base, int slots, const float* src) {
   const uint32_t slot = base + g % slots;
@@ -291,7 +262,7 @@ __device__ __forceinline__ void x_producer_loop(const SpadeArgs& a, const SynSme
     const float* base = a.x + static_cast<long>(b) * a.x_bstride + static_cast<long>(ti) * a.xC * 128;
     const float* base2 = a.x2 ? a.x2 + (static_cast<long>(b) * tm.T + ti) * a.xC * 128 : nullptr;
     for (int j = 0; j < 2 * a.nkc; ++j)
-      ring_emit(m, g, 0, kXs, (j < per_src ? base : base2 - per_src * 32 * 128) + j * 32 * 128);
+      ring_emit(m, g, 0, m.xs_n, (j < per_src ? base : base2 - per_src * 32 * 128) + j * 32 * 128);
   }
 }
 __device__ __forceinline__ void skip_producer_loop(const SpadeArgs& a, const SynSmem& m, const TileMap& tm) {
@@ -301,337 +272,268 @@ __device__ __forceinline__ void skip_producer_loop(const SpadeArgs& a, const Syn
     int b, ti;
     tm.get(it, b, ti);
     const float* base = a.skip + static_cast<long>(b) * a.skip_bstride + static_cast<long>(ti) * a.cout * 128;
-    for (int j = 0; j < a.cout / 32; ++j) ring_emit(m, g, kXs, kSs, base + j * 32 * 128);
+    for (int j = 0; j < a.cout / 32; ++j) ring_emit(m, g, m.xs_n, m.ss_n, base + j * 32 * 128);
   }
 }
 
-// Operand-team side of the activation ring: every warp walks both slices of a chunk, half h reads slice 2kc+h.
-__device__ __forceinline__ void take_x_pair(const SynSmem& m, uint32_t& xg, int h, int row, int lane, float (&dst)[32]) {
+// Ring protocol: every warp of both warpgroups waits for and releases EVERY slice in order (a warp reads only what it
+// needs).  With per-half arrivals a slot of an odd-sized ring alternates between halves, a fast half gets two phases
+// ahead and the parity wait succeeds on a stale phase.
+__device__ __forceinline__ uint32_t ring_take(const SynSmem& m, uint32_t g, int base, int slots) {
+  const uint32_t slot = base + g % slots;
+  mbar_wait_sleep(m.bars + X_FULL + slot, (g / slots) & 1);
+  return slot;
+}
+__device__ __forceinline__ void ring_release(const SynSmem& m, uint32_t slot) {
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) mbar_arrive(m.bars + X_EMPTY + slot);
+}
+
+// Operand-side read of a chunk's two activation slices in the row layout: half h reads slice 2kc+h.
+__device__ __forceinline__ void take_x_pair(const SynSmem& m, uint32_t& xg, int h, int row, float (&dst)[32]) {
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh, ++xg) {
-    const uint32_t xslot = xg % kXs;
-    mbar_wait_sleep(m.bars + X_FULL + xslot, (xg / kXs) & 1);
+    const uint32_t xslot = ring_take(m, xg, 0, m.xs_n);
     if (hh == h) {
       const uint32_t xs = smem_u32(m.x_st + xslot * (kXSlice / 4)) + row * 4;
 #pragma unroll
       for (int j = 0; j < 32; ++j) dst[j] = lds_f32(xs + j * 512);
     }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(m.bars + X_EMPTY + xslot);
+    ring_release(m, xslot);
   }
 }
 
-// ------------------------------------------------------------------------------------------
-// warps 8-11: epilogue team (identical for both variants): tile `it` lives in TMEM half it&1.
-// The four epilogue warps -- one per scheduler, each a single instruction stream -- are the critical path of these
-// kernels (ncu: never waiting, ~5 cycles per instruction), so the per-element work is straight-line code: residual /
-// ToRGB / statistics are compile-time variants and rows past the image are handled by one warp-uniform branch per
-// 32-column group (with run-time flags inside the unrolled loop the plain half-block spent 391 instructions per group,
-// 45 % of them selects, zero-adds, register clears and branches).
-// ------------------------------------------------------------------------------------------
-template <bool kSkip, bool kRgb, bool kStats>
-__device__ __forceinline__ void epilogue_team_variant(const SpadeArgs& a, const SynSmem& m, const TileMap& tm, uint32_t tmem,
-                                                      int q, int lane) {
-  const int row = q * 32 + lane;
-  uint32_t sg = 0;   // residual slices consumed
-  uint32_t tbias = smem_u32(m.tab_bias), trgb = smem_u32(m.tab_rgbw);   // constant tables, written before init's barrier
-  opaque(tbias);
-  opaque(trgb);
-  // without a residual the 2 residual staging slots (32 KB) are free: per-warp [32][33] transpose scratch for the
-  // statistics (32 STS + 32 LDS + 64 FP instead of a 248-instruction shuffle tree)
-  const uint32_t scratch = smem_u32(m.x_st + kXs * (kXSlice / 4) + q * (32 * 33));
-  const int HW = a.HW, cout = a.cout, ncg = a.cout >> 5;
-  float* const outp = a.out;
-  for (int it = 0; it < tm.count; ++it) {
-    int b, ti;
-    tm.get(it, b, ti);
-    const uint32_t buf = it & 1;
-    const int pix = ti * 128 + row;
-    const bool valid = pix < HW;
-    const bool full = ti * 128 + 128 <= HW;      // warp-uniform: every row of the tile is a pixel
-    float* const orow = outp + (static_cast<long>(b) * tm.T + ti) * cout * 128 + row;
-    mbar_wait_sleep(m.bars + ACC_FULL + buf, (it >> 1) & 1);
-    tc_fence_after();
-    float2 r0 = make_float2(0.f, 0.f), r1 = r0, r2 = r0;
-#pragma unroll 1
-    for (int cg = 0; cg < ncg; ++cg) {
-      const int c0 = cg * 32;
-      uint32_t raw[32];
-      tmem_ld32(tmem + buf * 256 + (static_cast<uint32_t>(q * 32) << 16) + c0, raw);
-      float sk[32];
-      if (kSkip) {
-        const uint32_t sslot = kXs + sg % kSs;
-        mbar_wait_sleep(m.bars + X_FULL + sslot, (sg / kSs) & 1);
-        const uint32_t xs = smem_u32(m.x_st + sslot * (kXSlice / 4)) + row * 4;
+// Column sums over the 64 rows of a warpgroup's fragments, folded into the CTA's shared sums: v[jj][e] holds this
+// thread's two rows of column 8 j + 2 (t%4) + e; lanes with equal t%4 hold the same columns.
+__device__ __forceinline__ void column_sums(float* st, int c0, const float (&v)[4][2]) {
 #pragma unroll
-        for (int j = 0; j < 32; ++j) sk[j] = lds_f32(xs + j * 512);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(m.bars + X_EMPTY + sslot);
-        ++sg;
-      }
-      tmem_ld_wait();
-      float v[32];
+  for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        float bs[8];
-        lds8(tbias + (c0 + g * 8) * 4, bs);
-#pragma unroll
-        for (int jj = 0; jj < 8; jj += 2) {      // packed fp32 adds on channel pairs (same operations, half the instructions)
-          const int j = g * 8 + jj;
-          float2 p = __fadd2_rn(make_float2(__uint_as_float(raw[j]), __uint_as_float(raw[j + 1])), make_float2(bs[jj], bs[jj + 1]));
-          if (kSkip) p = __fadd2_rn(p, make_float2(sk[j], sk[j + 1]));
-          v[j] = p.x;
-          v[j + 1] = p.y;
-        }
-      }
-      float* const o = orow + c0 * 128;
-      if (full) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) o[j * 128] = v[j];
-      } else {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          if (valid) o[j * 128] = v[j];
-          else v[j] = 0.f;
-        }
-      }
-      if (kRgb) {
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          float w0[8], w1[8], w2[8];
-          lds8(trgb + (c0 + g * 8) * 4, w0);
-          lds8(trgb + (kC + c0 + g * 8) * 4, w1);
-          lds8(trgb + (2 * kC + c0 + g * 8) * 4, w2);
-#pragma unroll
-          for (int jj = 0; jj < 8; jj += 2) {      // even / odd channels in the two lanes of a packed accumulator
-            const float2 vv = make_float2(v[g * 8 + jj], v[g * 8 + jj + 1]);
-            r0 = __ffma2_rn(vv, make_float2(w0[jj], w0[jj + 1]), r0);
-            r1 = __ffma2_rn(vv, make_float2(w1[jj], w1[jj + 1]), r1);
-            r2 = __ffma2_rn(vv, make_float2(w2[jj], w2[jj + 1]), r2);
-          }
-        }
-      }
-      if (kStats) {
-        float t1, t2;
-        if (kSkip) {
-          float s2[32];
-#pragma unroll
-          for (int j = 0; j < 32; ++j) s2[j] = v[j] * v[j];
-          t1 = transpose_reduce32(v, lane);
-          t2 = transpose_reduce32(s2, lane);
-        } else {
-          __syncwarp();
-#pragma unroll
-          for (int j = 0; j < 32; ++j) asm volatile("st.shared.f32 [%0], %1;" ::"r"(scratch + (lane * 33 + j) * 4), "f"(v[j]) : "memory");
-          __syncwarp();
-          float2 ts = make_float2(0.f, 0.f), qs = make_float2(0.f, 0.f);      // two chains each, as one packed pair
-#pragma unroll
-          for (int r = 0; r < 32; r += 2) {
-            const float2 x = make_float2(lds_f32(scratch + (r * 33 + lane) * 4), lds_f32(scratch + ((r + 1) * 33 + lane) * 4));
-            ts = __fadd2_rn(ts, x);
-            qs = __ffma2_rn(x, x, qs);
-          }
-          t1 = ts.x + ts.y;
-          t2 = qs.x + qs.y;
-        }
-        atomicAdd(m.st_sum + c0 + lane, t1);
-        atomicAdd(m.st_sq + c0 + lane, t2);
-      }
+    for (int e = 0; e < 2; ++e) {
+      float x = v[jj][e];
+      x += __shfl_xor_sync(0xffffffffu, x, 4);
+      x += __shfl_xor_sync(0xffffffffu, x, 8);
+      x += __shfl_xor_sync(0xffffffffu, x, 16);
+      if ((threadIdx.x & 31) < 4) atomicAdd(st + c0 + 8 * jj + 2 * (threadIdx.x & 3) + e, x);
     }
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(m.bars + ACC_EMPTY + buf);
-    if (kRgb && valid) {   // this thread saw all 256 channels of its pixel
-      const float r[3] = {r0.x + r0.y, r1.x + r1.y, r2.x + r2.y};
+}
+
+// ------------------------------------------------------------------------------------------
+// Forward epilogue of one tile from the fragments of warpgroup g.  The residual is a compile-time variant; ToRGB and the
+// statistics are warp-uniform branches (eight fully unrolled variants took ptxas ten minutes for this file).
+// ------------------------------------------------------------------------------------------
+template <bool kSkip>
+__device__ __forceinline__ void epilogue_fwd(const SpadeArgs& a, const SynSmem& m, const float (&d)[128], int b, int ti, int T,
+                                             int g, int t, uint32_t& sg) {
+  const int HW = a.HW, cout = a.cout;
+  const bool kRgb = a.rgb_w != nullptr, kStats = a.stats != nullptr;
+  int row[2];
+  bool valid[2];
 #pragma unroll
-      for (int j = 0; j < 3; ++j) {
-        const long idx = (static_cast<long>(b) * 3 + j) * HW + pix;
-        float o = r[j] + a.rgb_b[j];
-        if (a.rgb_in) o += a.rgb_in[idx];
-        a.rgb_out[idx] = o;
+  for (int i = 0; i < 2; ++i) {
+    row[i] = g * 64 + frag_row(t, i);
+    valid[i] = ti * 128 + row[i] < HW;
+  }
+  float* const otile = a.out + (static_cast<long>(b) * T + ti) * cout * 128;
+  float r[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+#pragma unroll
+  for (int cg = 0; cg < 8; ++cg) {
+    if (cg * 32 >= cout) break;
+    float sk[2][4][2];
+    if (kSkip) {
+      const uint32_t slot = ring_take(m, sg, m.xs_n, m.ss_n);
+      const float* xs = m.x_st + slot * (kXSlice / 4);
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) sk[i][jj][e] = xs[(frag_col(t, jj, e)) * 128 + row[i]];
+      ring_release(m, slot);
+      ++sg;
+    }
+    float s1[4][2], s2[4][2];
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int j = cg * 4 + jj, c = frag_col(t, j, e);
+        const float bc = m.tab_bias[c];
+        s1[jj][e] = 0.f;
+        s2[jj][e] = 0.f;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          float v = d[4 * j + 2 * i + e] + bc;
+          if (kSkip) v += sk[i][jj][e];
+          if (valid[i]) otile[c * 128 + row[i]] = v;
+          else v = 0.f;
+          if (kRgb) {
+#pragma unroll
+            for (int k = 0; k < 3; ++k) r[i][k] = fmaf(v, m.tab_rgbw[k * kC + c], r[i][k]);
+          }
+          s1[jj][e] += v;
+          s2[jj][e] = fmaf(v, v, s2[jj][e]);
+        }
       }
+    if (kStats) {
+      column_sums(m.st_sum, cg * 32, s1);
+      column_sums(m.st_sq, cg * 32, s2);
     }
   }
-  asm volatile("bar.sync 2, 128;" ::: "memory");
-  if (kStats) {
-    for (int c = threadIdx.x - 256; c < kC; c += 128) {
-      atomicAdd(a.stats + c, static_cast<double>(m.st_sum[c]));
-      atomicAdd(a.stats + kC + c, static_cast<double>(m.st_sq[c]));
+  if (kRgb) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+#pragma unroll
+      for (int k = 0; k < 3; ++k) {
+        r[i][k] += __shfl_xor_sync(0xffffffffu, r[i][k], 1);
+        r[i][k] += __shfl_xor_sync(0xffffffffu, r[i][k], 2);
+      }
+      if ((t & 3) == 0 && valid[i]) {
+        const int pix = ti * 128 + row[i];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+          const long idx = (static_cast<long>(b) * 3 + k) * HW + pix;
+          float o = r[i][k] + a.rgb_b[k];
+          if (a.rgb_in) o += a.rgb_in[idx];
+          a.rgb_out[idx] = o;
+        }
+      }
     }
   }
 }
 
 // warp-uniform dispatch on the launch's flags
-__device__ __forceinline__ void epilogue_team_loop(const SpadeArgs& a, const SynSmem& m, const TileMap& tm, uint32_t tmem,
-                                                   int q, int lane) {
-  const int sel = (a.skip ? 4 : 0) | (a.rgb_w ? 2 : 0) | (a.stats ? 1 : 0);
-  switch (sel) {
-    case 0: epilogue_team_variant<false, false, false>(a, m, tm, tmem, q, lane); break;
-    case 1: epilogue_team_variant<false, false, true>(a, m, tm, tmem, q, lane); break;
-    case 2: epilogue_team_variant<false, true, false>(a, m, tm, tmem, q, lane); break;
-    case 3: epilogue_team_variant<false, true, true>(a, m, tm, tmem, q, lane); break;
-    case 4: epilogue_team_variant<true, false, false>(a, m, tm, tmem, q, lane); break;
-    case 5: epilogue_team_variant<true, false, true>(a, m, tm, tmem, q, lane); break;
-    case 6: epilogue_team_variant<true, true, false>(a, m, tm, tmem, q, lane); break;
-    default: epilogue_team_variant<true, true, true>(a, m, tm, tmem, q, lane); break;
-  }
+__device__ __forceinline__ void epilogue_fwd_any(const SpadeArgs& a, const SynSmem& m, const float (&d)[128], int b, int ti, int T,
+                                                 int g, int t, uint32_t& sg) {
+  if (a.skip) epilogue_fwd<true>(a, m, d, b, ti, T, g, t, sg);
+  else epilogue_fwd<false>(a, m, d, b, ti, T, g, t, sg);
 }
 
+// the forward statistics of the CTA -> the launch's [2,C] fp64 sums (after every tile's column_sums)
+__device__ __forceinline__ void flush_fwd_stats(const SpadeArgs& a, const SynSmem& m) {
+  rows_barrier();
+  if (a.stats)
+    for (int c = threadIdx.x; c < kC; c += 256) {
+      atomicAdd(a.stats + c, static_cast<double>(m.st_sum[c]));
+      atomicAdd(a.stats + kC + c, static_cast<double>(m.st_sq[c]));
+    }
+}
 
 // ------------------------------------------------------------------------------------------
-// warps 8-11 of the BACKWARD (data-gradient) variant.  The accumulator holds dL/dy = W^T dL/dout for the 128
+// Epilogue of the BACKWARD (data-gradient) variant.  The accumulator holds dL/dy = W^T dL/dout for the 128
 // pixels of the tile; the forward input x of the half-block arrives through the residual ring, so that
 //     pre = x*g1[b,c] + g0[b,c]            (the folded BatchNorm + SPADE modulation of the forward pass)
 //     dpre = dL/dy * lrelu'(pre)           -> stored (tile-blocked, like every activation)
 //     S1[b,c] += dpre,  S2[b,c] += dpre*x  -> everything BatchNorm / gamma / beta need (DESIGN.md "Backward")
-// ------------------------------------------------------------------------------------------
-// Compile-time variants (the per-element work must be straight-line code: with run-time flags inside the 32-wide unrolled
-// loop the compiler emitted ~4 branches, 4 address LEAs and several constant reloads per element, and the four epilogue
-// warps -- one instruction stream per scheduler -- became the critical path of the kernel at 5.7 cycles per instruction):
+// Compile-time variants (straight-line per-element code):
 //   kSine  activation derivative cos(pre) (FiLM-SIREN) instead of the LeakyReLU / ReLU mask
 //   kRk    rank-3 term from the renderer's heads (rows beyond rk_n of the [3,C] weight table are zero)
 //   kPm    pixel-major [B,HW,cout] output
+// The per-sample tables tab_g1 / tab_g0 and sums st_sum / st_sq are managed by the caller.
+// ------------------------------------------------------------------------------------------
 template <bool kSine, bool kRk, bool kPm>
-__device__ __forceinline__ void epilogue_bwd_loop(const SpadeArgs& a, const SynSmem& m, const TileMap& tm, uint32_t tmem,
-                                                  int q, int lane) {
-  const int row = q * 32 + lane;
-  const int et = threadIdx.x - 256;   // 0..127 within the epilogue team
-  uint32_t sg = 0;
-  int cur_b = -1;
-  const int cout = a.cout;
-  double* const stats = a.stats;
-  auto flush = [&](int b) {
-    for (int c = et; c < cout; c += 128) {
-      atomicAdd(stats + (static_cast<long>(b) * 2 + 0) * cout + c, static_cast<double>(m.st_sum[c]));
-      atomicAdd(stats + (static_cast<long>(b) * 2 + 1) * cout + c, static_cast<double>(m.st_sq[c]));
-      m.st_sum[c] = 0.f;
-      m.st_sq[c] = 0.f;
-    }
-  };
+__device__ __forceinline__ void epilogue_bwd(const SpadeArgs& a, const SynSmem& m, const float (&d)[128], int b, int ti, int T, int g,
+                                             int t, uint32_t& sg) {
+  const int HW = a.HW, cout = a.cout, rk_n = a.rk_n;
   const float mslope = a.slope;
-  const int ncg = cout >> 5;
-  const int HW = a.HW, rk_n = a.rk_n;
-  const float* const modp = a.mod;
-  const float* const rkv = a.rk_v;
-  float* const outp = a.out;
-  uint32_t trk = smem_u32(m.tab_rgbw);     // rank-k weights (loaded by init_common through a.rgb_w)
-  opaque(trk);
-  for (int it = 0; it < tm.count; ++it) {
-    int b, ti;
-    tm.get(it, b, ti);
-    if (b != cur_b) {   // per-sample tables and per-sample sums
-      asm volatile("bar.sync 2, 128;" ::: "memory");
-      if (cur_b >= 0) flush(cur_b);
-      for (int c = et; c < cout; c += 128) {
-        m.tab_g1[c] = modp ? modp[(static_cast<long>(b) * 2 + 0) * cout + c] : 1.f;
-        m.tab_g0[c] = modp ? modp[(static_cast<long>(b) * 2 + 1) * cout + c] : 0.f;
-      }
-      asm volatile("bar.sync 2, 128;" ::: "memory");
-      cur_b = b;
+  int row[2];
+  bool valid[2];
+  float rv[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    row[i] = g * 64 + frag_row(t, i);
+    valid[i] = ti * 128 + row[i] < HW;
+    if (kRk && valid[i]) {
+      const float* rp = a.rk_v + static_cast<long>(b) * rk_n * HW + ti * 128 + row[i];
+      rv[i][0] = rp[0];
+      if (rk_n > 1) rv[i][1] = rp[HW];
+      if (rk_n > 2) rv[i][2] = rp[2 * static_cast<long>(HW)];
     }
-    uint32_t tg1 = smem_u32(m.tab_g1), tg0 = smem_u32(m.tab_g0);
-    opaque(tg1);   // no table load may move above the refresh
-    opaque(tg0);
-    const uint32_t buf = it & 1;
-    const bool valid = ti * 128 + row < HW;
-    float* const orow = kPm ? outp + (static_cast<long>(b) * HW + ti * 128 + row) * cout
-                            : outp + (static_cast<long>(b) * tm.T + ti) * cout * 128 + row;
-    float rv0 = 0.f, rv1 = 0.f, rv2 = 0.f;
-    if (kRk && valid) {
-      const float* r = rkv + static_cast<long>(b) * rk_n * HW + ti * 128 + row;
-      rv0 = r[0];
-      if (rk_n > 1) rv1 = r[HW];
-      if (rk_n > 2) rv2 = r[2 * static_cast<long>(HW)];
-    }
-    mbar_wait_sleep(m.bars + ACC_FULL + buf, (it >> 1) & 1);
-    tc_fence_after();
-#pragma unroll 1
-    for (int cg = 0; cg < ncg; ++cg) {
-      const int c0 = cg * 32;
-      uint32_t raw[32];
-      tmem_ld32(tmem + buf * 256 + (static_cast<uint32_t>(q * 32) << 16) + c0, raw);
-      float xs_[32];
-      {
-        const uint32_t sslot = kXs + sg % kSs;
-        mbar_wait_sleep(m.bars + X_FULL + sslot, (sg / kSs) & 1);
-        const uint32_t xs = smem_u32(m.x_st + sslot * (kXSlice / 4)) + row * 4;
-#pragma unroll
-        for (int j = 0; j < 32; ++j) xs_[j] = lds_f32(xs + j * 512);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(m.bars + X_EMPTY + sslot);
-        ++sg;
-      }
-      if (!valid) {      // rows past the image (last, partial tile only): the staged slice holds whatever the padding holds
-#pragma unroll
-        for (int j = 0; j < 32; ++j) xs_[j] = 0.f;
-      }
-      tmem_ld_wait();
-      float v[32], w[32];
-      float* const o = kPm ? orow + c0 : orow + c0 * 128;
-#pragma unroll
-      for (int g = 0; g < 4; ++g) {
-        float t1[8], t0[8], k0[8], k1[8], k2[8];
-        lds8(tg1 + (c0 + g * 8) * 4, t1);
-        lds8(tg0 + (c0 + g * 8) * 4, t0);
-        if (kRk) {
-          lds8(trk + (c0 + g * 8) * 4, k0);
-          lds8(trk + (kC + c0 + g * 8) * 4, k1);
-          lds8(trk + (2 * kC + c0 + g * 8) * 4, k2);
-        }
-#pragma unroll
-        for (int jj = 0; jj < 8; jj += 2) {      // channel pairs on packed fp32 (same operations)
-          const int j = g * 8 + jj;
-          const float2 x2 = make_float2(xs_[j], xs_[j + 1]);
-          const float2 pre = __ffma2_rn(x2, make_float2(t1[jj], t1[jj + 1]), make_float2(t0[jj], t0[jj + 1]));
-          float2 acc = make_float2(__uint_as_float(raw[j]), __uint_as_float(raw[j + 1]));   // 0 for rows past the image
-          if (kRk) {
-            const float2 a0 = make_float2(rv0, rv0), a1 = make_float2(rv1, rv1), a2 = make_float2(rv2, rv2);
-            acc = __ffma2_rn(a2, make_float2(k2[jj], k2[jj + 1]),
-                             __ffma2_rn(a1, make_float2(k1[jj], k1[jj + 1]), __ffma2_rn(a0, make_float2(k0[jj], k0[jj + 1]), acc)));
-          }
-          const float2 mask = kSine ? cos_red2(pre)
-                                    : make_float2(pre.x > 0.f ? 1.f : mslope, pre.y > 0.f ? 1.f : mslope);
-          const float2 d = __fmul2_rn(acc, mask);
-          const float2 dx = __fmul2_rn(d, x2);
-          if (!kPm && valid) {
-            o[j * 128] = d.x;
-            o[(j + 1) * 128] = d.y;
-          }
-          v[j] = d.x;
-          v[j + 1] = d.y;
-          w[j] = dx.x;
-          w[j + 1] = dx.y;
-        }
-      }
-      if (kPm && valid) {
-        float4* o4 = reinterpret_cast<float4*>(o);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) o4[j] = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-      }
-      const float s1 = transpose_reduce32(v, lane);
-      const float s2 = transpose_reduce32(w, lane);
-      atomicAdd(m.st_sum + c0 + lane, s1);
-      atomicAdd(m.st_sq + c0 + lane, s2);
-    }
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) mbar_arrive(m.bars + ACC_EMPTY + buf);
   }
-  asm volatile("bar.sync 2, 128;" ::: "memory");
-  if (cur_b >= 0) flush(cur_b);
+  float* const otile = a.out + (static_cast<long>(b) * T + ti) * cout * 128;
+#pragma unroll
+  for (int cg = 0; cg < 8; ++cg) {
+    if (cg * 32 >= cout) break;
+    float xv[2][4][2];
+    {
+      const uint32_t slot = ring_take(m, sg, m.xs_n, m.ss_n);
+      const float* xs = m.x_st + slot * (kXSlice / 4);
+#pragma unroll
+      for (int i = 0; i < 2; ++i)
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+          for (int e = 0; e < 2; ++e)   // rows past the image (last, partial tile only): the slice holds whatever the padding holds
+            xv[i][jj][e] = valid[i] ? xs[frag_col(t, jj, e) * 128 + row[i]] : 0.f;
+      ring_release(m, slot);
+      ++sg;
+    }
+    float s1[4][2], s2[4][2];
+#pragma unroll
+    for (int jj = 0; jj < 4; ++jj)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int j = cg * 4 + jj, c = frag_col(t, j, e);
+        const float t1 = m.tab_g1[c], t0 = m.tab_g0[c];
+        s1[jj][e] = 0.f;
+        s2[jj][e] = 0.f;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const float x = xv[i][jj][e];
+          const float pre = fmaf(x, t1, t0);
+          float acc = d[4 * j + 2 * i + e];       // 0 for rows past the image
+          if (kRk)
+            acc = fmaf(rv[i][2], m.tab_rgbw[2 * kC + c], fmaf(rv[i][1], m.tab_rgbw[kC + c], fmaf(rv[i][0], m.tab_rgbw[c], acc)));
+          const float mask = kSine ? cos_red(pre) : (pre > 0.f ? 1.f : mslope);
+          const float dd = acc * mask;
+          if (valid[i]) {
+            if (kPm) a.out[(static_cast<long>(b) * HW + ti * 128 + row[i]) * cout + c] = dd;
+            else otile[c * 128 + row[i]] = dd;
+          }
+          s1[jj][e] += dd;
+          s2[jj][e] = fmaf(dd, x, s2[jj][e]);
+        }
+      }
+    column_sums(m.st_sum, cg * 32, s1);
+    column_sums(m.st_sq, cg * 32, s2);
+  }
+}
+
+__device__ __forceinline__ void epilogue_bwd_any(const SpadeArgs& a, const SynSmem& m, const float (&d)[128], int b, int ti, int T,
+                                                 int g, int t, uint32_t& sg) {
+  // warp-uniform dispatch to a straight-line variant (the host side rejects the other combinations)
+  if (a.act == 1) {
+    if (a.rk_v) epilogue_bwd<true, true, false>(a, m, d, b, ti, T, g, t, sg);
+    else epilogue_bwd<true, false, false>(a, m, d, b, ti, T, g, t, sg);
+  } else {
+    if (a.out_pm) epilogue_bwd<false, false, true>(a, m, d, b, ti, T, g, t, sg);
+    else epilogue_bwd<false, false, false>(a, m, d, b, ti, T, g, t, sg);
+  }
+}
+
+// per-sample sums of the backward variant -> stats [B,2,cout] (fp64), then cleared
+__device__ __forceinline__ void flush_bwd_sums(const SpadeArgs& a, const SynSmem& m, int b) {
+  for (int c = threadIdx.x; c < a.cout; c += 256) {
+    atomicAdd(a.stats + (static_cast<long>(b) * 2 + 0) * a.cout + c, static_cast<double>(m.st_sum[c]));
+    atomicAdd(a.stats + (static_cast<long>(b) * 2 + 1) * a.cout + c, static_cast<double>(m.st_sq[c]));
+    m.st_sum[c] = 0.f;
+    m.st_sq[c] = 0.f;
+  }
 }
 
 // ------------------------------------------------------------------------------------------
-// const-style variant.  kBwd: data gradient of the same half-block: the operand is dL/dout passed through
-// unchanged, the weight image is W^T, the epilogue is `epilogue_bwd_loop`.
+// const-style variant (384 threads).  Warpgroup g (warps 4g..4g+3) builds rows 64g..64g+63 of each K chunk in a 2-slot
+// ring (warp (q, h): rows 32q.., channels 32h.. of the chunk), issues their wgmmas ([64 x 256] fp32 accumulator in
+// registers) and runs the epilogue; warp 8 streams the weights, warp 9 the activation slices, warp 10 the residual slices.
+// kBwd: data gradient of the same half-block: the operand is dL/dout passed through unchanged (optionally scaled), the
+// weight image is W^T, the epilogue is `epilogue_bwd`.
 // ------------------------------------------------------------------------------------------
 template <int kPasses, bool kBwd>
 __global__ void __launch_bounds__(kSynThreads, 1) spade_const_kernel(SpadeArgs a) {
   extern __shared__ uint8_t smem_raw[];
-  const SynSmem m = carve(smem_raw);
+  const SynSmem m = carve<false>(smem_raw);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  init_common(a, m, warp);
-  const uint32_t tmem = *m.tmem_slot;
+  init_common(a, m);
   TileMap tm;
   tm.T = (a.HW + 127) / 128;
   tm.first = blockIdx.x;
@@ -639,20 +541,28 @@ __global__ void __launch_bounds__(kSynThreads, 1) spade_const_kernel(SpadeArgs a
   tm.count = (a.B * tm.T - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);
 
   if (warp < 8) {
-    // ------------------------------------------------------------------ operand team
-    const int q = warp & 3, h = warp >> 2;
+    regs_inc<kMmaRegs>();
+    const int g = warp >> 2, t = threadIdx.x & 127;
+    const int q = 2 * g + (warp & 1), h = (warp >> 1) & 1;
     const int row = q * 32 + lane;
     int cur_b = -1;
     uint32_t acnt = 0;   // operand chunks produced (2-slot ring)
-    uint32_t xg = 0;     // activation slices walked
+    uint32_t xg = 0, sg = 0;
+    Pipe p;
+    float d[128];
     for (int it = 0; it < tm.count; ++it) {
       int b, ti;
       tm.get(it, b, ti);
-      if (b != cur_b && (!kBwd || a.ascale)) {  // refresh the per-sample tables of the operand team
+      if (b != cur_b) {  // refresh the per-sample tables (and, backward, flush the previous sample's sums)
         rows_barrier();
+        if (kBwd && cur_b >= 0) flush_bwd_sums(a, m, cur_b);
         for (int i = threadIdx.x; i < kC; i += 256) {
           if (kBwd) {
-            m.tab_as[i] = a.ascale[static_cast<long>(b) * kC + i];
+            if (a.ascale) m.tab_as[i] = a.ascale[static_cast<long>(b) * kC + i];
+            if (i < a.cout) {
+              m.tab_g1[i] = a.mod ? a.mod[(static_cast<long>(b) * 2 + 0) * a.cout + i] : 1.f;
+              m.tab_g0[i] = a.mod ? a.mod[(static_cast<long>(b) * 2 + 1) * a.cout + i] : 0.f;
+            }
           } else {   // no table = identity (plain 1x1 convolution)
             m.tab_g1[i] = a.mod ? a.mod[(static_cast<long>(b) * 2 + 0) * kC + i] : 1.f;
             m.tab_g0[i] = a.mod ? a.mod[(static_cast<long>(b) * 2 + 1) * kC + i] : 0.f;
@@ -681,86 +591,57 @@ __global__ void __launch_bounds__(kSynThreads, 1) spade_const_kernel(SpadeArgs a
         const bool second = two_tables && kc * 64 >= kC;
         const uint32_t tg1 = second ? tg1b : tg1a, tg0 = second ? tg0b : tg0a;
         float cur[32];
-        take_x_pair(m, xg, h, row, lane, cur);
+        take_x_pair(m, xg, h, row, cur);
+        // the slot was last read by chunk acnt - 2, whose wgmmas pipe_chunk has seen complete
         const uint32_t slot = acnt & 1;
-        mbar_wait_sleep(m.bars + A_EMPTY + slot, ((acnt >> 1) & 1) ^ 1);
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
+        for (int gi = 0; gi < 4; ++gi) {
           float y[8], t1[8], t0[8];
-          if (!kBwd || scaled) lds8(tg1 + (c0 + g * 8) * 4, t1);
-          if (!kBwd) lds8(tg0 + (c0 + g * 8) * 4, t0);
+          if (!kBwd || scaled) lds8(tg1 + (c0 + gi * 8) * 4, t1);
+          if (!kBwd) lds8(tg0 + (c0 + gi * 8) * 4, t0);
           if (kBwd) {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) y[j] = scaled ? cur[g * 8 + j] * t1[j] : cur[g * 8 + j];
+            for (int j = 0; j < 8; ++j) y[j] = scaled ? cur[gi * 8 + j] * t1[j] : cur[gi * 8 + j];
           } else if (sine) {
 #pragma unroll
             for (int j = 0; j < 8; j += 2) {
-              const float2 sv = sin_red2(__ffma2_rn(make_float2(cur[g * 8 + j], cur[g * 8 + j + 1]), make_float2(t1[j], t1[j + 1]),
-                                                    make_float2(t0[j], t0[j + 1])));
+              const float2 sv = sin_red2(ffma2(make_float2(cur[gi * 8 + j], cur[gi * 8 + j + 1]), make_float2(t1[j], t1[j + 1]),
+                                               make_float2(t0[j], t0[j + 1])));
               y[j] = sv.x;
               y[j + 1] = sv.y;
             }
           } else {
-            affine_lrelu8(cur + g * 8, t1, t0, slope, y);
+            affine_lrelu8(cur + gi * 8, t1, t0, slope, y);
           }
           if (!valid) {   // only the last, partial tile of an image
 #pragma unroll
             for (int j = 0; j < 8; ++j) y[j] = 0.f;
           }
-          store_a8<kPasses == 3>(m.a_hi + slot * kAChunk, m.a_lo + slot * kAChunk, row, h * 32 + g * 8, y);
+          store_a8<kPasses == 3>(m.a_hi + slot * kAChunk, m.a_lo + slot * kAChunk, row, h * 32 + gi * 8, y);
         }
         fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(m.bars + A_FULL + slot);
+        named_barrier(2 + g, 128);
+        pipe_chunk<256, kPasses>(m, p, d, smem_u32(m.a_hi + slot * kAChunk) + g * 64 * 128,
+                                 smem_u32(m.a_lo + slot * kAChunk) + g * 64 * 128, kc > 0, t);
       }
+      pipe_drain<256>(m, p, d, t);
+      if (kBwd) epilogue_bwd_any(a, m, d, b, ti, tm.T, g, t, sg);
+      else epilogue_fwd_any(a, m, d, b, ti, tm.T, g, t, sg);
     }
-  } else if (warp < 12) {
-    if (kBwd) {      // warp-uniform dispatch to a straight-line variant (the host side rejects the other combinations)
-      if (a.act == 1) {
-        if (a.rk_v) epilogue_bwd_loop<true, true, false>(a, m, tm, tmem, warp - 8, lane);
-        else epilogue_bwd_loop<true, false, false>(a, m, tm, tmem, warp - 8, lane);
-      } else {
-        if (a.out_pm) epilogue_bwd_loop<false, false, true>(a, m, tm, tmem, warp - 8, lane);
-        else epilogue_bwd_loop<false, false, false>(a, m, tm, tmem, warp - 8, lane);
-      }
+    if (kBwd) {
+      rows_barrier();
+      if (cur_b >= 0) flush_bwd_sums(a, m, cur_b);
     } else {
-      epilogue_team_loop(a, m, tm, tmem, warp - 8, lane);
+      flush_fwd_stats(a, m);
     }
-  } else if (warp == 12) {
-    {
-      const bool leader = elect_one_sync();
-      const uint32_t idesc = umma_idesc_bf16(128, 256);
-      MmaPipe p;
-      uint32_t acnt = 0;
-      for (int it = 0; it < tm.count; ++it) {
-        const uint32_t buf = it & 1;
-        mbar_wait_sleep(m.bars + ACC_EMPTY + buf, ((it >> 1) & 1) ^ 1);
-        tc_fence_after();
-        for (int kc = 0; kc < a.nkc; ++kc, ++acnt) {
-          const uint32_t slot = acnt & 1;
-          mbar_wait_sleep(m.bars + A_FULL + slot, (acnt >> 1) & 1);
-          tc_fence_after();
-          mma_chunk<kPasses>(m, p, leader, tmem + buf * 256, smem_u32(m.a_hi + slot * kAChunk), smem_u32(m.a_lo + slot * kAChunk),
-                             idesc, kc > 0);
-          umma_commit_if(leader, m.bars + A_EMPTY + slot);
-        }
-        umma_commit_if(leader, m.bars + ACC_FULL + buf);
-      }
-    }
-  } else if (warp == 13) {
-    if (lane == 0) {
-      const uint8_t* imgs[1] = {a.wimg};
-      const int ns[1] = {2 * a.nkc};
-      weight_producer_loop<kPasses>(m, imgs, ns, 1, tm.count);
-    }
-  } else if (warp == 14) {
-    if (lane == 0) x_producer_loop(a, m, tm);
   } else {
-    if (lane == 0) skip_producer_loop(a, m, tm);
+    regs_dec<kProducerRegs>();
+    if (lane == 0) {
+      if (warp == 8) weight_producer_loop<kPasses>(m, a.wimg, 2 * a.nkc, tm.count);
+      else if (warp == 9) x_producer_loop(a, m, tm);
+      else if (warp == 10) skip_producer_loop(a, m, tm);
+    }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 12) tmem_dealloc<512>(tmem);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -776,18 +657,40 @@ __device__ __forceinline__ void bilin(int dst, int in_size, float scale, int& i0
   l0 = 1.f - l1;
 }
 
+// Weight stages of one pixel-style tile: per conv K chunk kc, the [gamma | beta] rows of channels 64kc.. (128 rows of
+// gamma/beta block kc/2) for both K chunks of A1, then the conv chunk kc.
+template <int kPasses>
+__device__ __forceinline__ void pixel_weight_producer_loop(const SpadeArgs& a, const SynSmem& m, int num_my_tiles) {
+  uint32_t st = 0, ph = 0;
+  auto emit = [&](const uint8_t* src, uint32_t bytes) {
+    mbar_wait_backoff(m.bars + B_EMPTY + st, ph ^ 1);
+    mbar_arrive_expect_tx(m.bars + B_FULL + st, bytes);
+    bulk_g2s(m.b_st + st * kBStage, src, bytes, m.bars + B_FULL + st);
+    if (++st == kSynStages) { st = 0; ph ^= 1; }
+  };
+  for (int t = 0; t < num_my_tiles; ++t)
+    for (int kc = 0; kc < 4; ++kc) {
+      for (int k = 0; k < 2; ++k)
+        for (int part = 0; part < (kPasses == 3 ? 2 : 1); ++part)
+          emit(a.wgb + static_cast<size_t>(((kc >> 1) * 2 + k) * 2 + part) * kBStage + (kc & 1) * (kBStage / 2), kBStage / 2);
+      for (int part = 0; part < (kPasses == 3 ? 2 : 1); ++part) emit(a.wimg + static_cast<size_t>(kc * 2 + part) * kBStage, kBStage);
+    }
+}
+
+// Per tile: A1 = relu(bilinear(P_lr) + c) (K = 128, two chunks); then per conv K chunk kc: [gamma | beta] of channels
+// 64kc.. = A1 . Wgb (a [64 x 128] accumulator per warpgroup), y = lrelu(BN(x)*(1+gamma)+beta) -> the y chunk, conv
+// accumulate.  The 28x larger up-sampled style map of map3d_generator.py:244-245 is never materialised.
 template <int kPasses>
 __global__ void __launch_bounds__(kSynThreads, 1) spade_pixel_kernel(SpadeArgs a) {
   extern __shared__ uint8_t smem_raw[];
-  const SynSmem m = carve(smem_raw);
+  const SynSmem m = carve<true>(smem_raw);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int i = threadIdx.x; i < kC; i += blockDim.x) {
     m.tab_g1[i] = a.scsh[i];
     m.tab_g0[i] = a.scsh[kC + i];
   }
   for (int i = threadIdx.x; i < 512; i += blockDim.x) m.tab_bgb[i] = a.bgb[i];
-  init_common(a, m, warp);
-  const uint32_t tmem = *m.tmem_slot;
+  init_common(a, m);
   TileMap tm;
   tm.T = (a.HW + 127) / 128;
   tm.first = blockIdx.x;
@@ -797,23 +700,21 @@ __global__ void __launch_bounds__(kSynThreads, 1) spade_pixel_kernel(SpadeArgs a
   const float sx = static_cast<float>(a.Rw) / static_cast<float>(a.Wg);
 
   if (warp < 8) {
-    // ------------------------------------------------------------------ operand team
-    const int q = warp & 3, h = warp >> 2;
+    regs_inc<kMmaRegs>();
+    const int g = warp >> 2, t = threadIdx.x & 127;
+    const int q = 2 * g + (warp & 1), h = (warp >> 1) & 1;
     const int row = q * 32 + lane;
-    uint32_t acnt = 0, xg = 0;
-    uint32_t tg1 = smem_u32(m.tab_g1), tg0 = smem_u32(m.tab_g0), tbgb = smem_u32(m.tab_bgb);   // constant tables
-    opaque(tg1);
-    opaque(tg0);
-    opaque(tbgb);
+    uint8_t* const y_hi = m.a_hi + 2 * kAChunk;
+    uint8_t* const y_lo = m.a_lo + 2 * kAChunk;
+    uint32_t xg = 0, sg = 0;
+    Pipe p;
+    float d[128], e[64];
     for (int it = 0; it < tm.count; ++it) {
       int b, ti;
       tm.get(it, b, ti);
       const int pix = ti * 128 + row;
       const bool valid = pix < a.HW;
-      const uint32_t R = (it & 1) * 256, Rp = 256 - R;      // TMEM halves of this tile
-      // ---- phase 0: A1 = relu(bilinear(P_lr) + c): column half h builds K chunk h into ring slot h.
-      // Both slots must have been consumed by the previous tile's conv (its chunks 2 and 3).
-      if (it > 0) mbar_wait_sleep(m.bars + A_EMPTY + h, 1);
+      // ---- A1 = relu(bilinear(P_lr) + c): column half h builds K chunk h (the previous tile's wgmmas are complete)
       {
         const int py = valid ? pix / a.Wg : 0, px = valid ? pix % a.Wg : 0;
         int y0, y1, x0, x1;
@@ -828,135 +729,94 @@ __global__ void __launch_bounds__(kSynThreads, 1) spade_pixel_kernel(SpadeArgs a
         const float4* pb = a.p_bias ? reinterpret_cast<const float4*>(a.p_bias + static_cast<long>(b) * 128) : nullptr;
         const float2 lx0p = make_float2(lx0, lx0), lx1p = make_float2(lx1, lx1), ly0p = make_float2(ly0, ly0), ly1p = make_float2(ly1, ly1);
 #pragma unroll 2
-        for (int g = 0; g < 8; ++g) {
+        for (int gi = 0; gi < 8; ++gi) {
           float y[8];
 #pragma unroll
           for (int u = 0; u < 2; ++u) {
-            const int f4 = h * 16 + g * 2 + u;
+            const int f4 = h * 16 + gi * 2 + u;
             const float4 v00 = __ldg(n00 + f4), v01 = __ldg(n01 + f4), v10 = __ldg(n10 + f4), v11 = __ldg(n11 + f4);
-            // same association as upsample_bilinear2d: ly0*(lx0*a + lx1*b) + ly1*(lx0*c + lx1*d), on channel pairs (packed fp32:
-            // this loop is on the critical chain of the tile -- the gamma/beta GEMM cannot start before it)
+            // same association as upsample_bilinear2d: ly0*(lx0*a + lx1*b) + ly1*(lx0*c + lx1*d), on channel pairs
             auto lerp2 = [&](float2 a, float2 b, float2 c, float2 d) {
-              const float2 top = __ffma2_rn(b, lx1p, __fmul2_rn(a, lx0p));
-              const float2 bot = __ffma2_rn(d, lx1p, __fmul2_rn(c, lx0p));
-              return __ffma2_rn(top, ly0p, __fmul2_rn(bot, ly1p));
+              const float2 top = ffma2(b, lx1p, fmul2(a, lx0p));
+              const float2 bot = ffma2(d, lx1p, fmul2(c, lx0p));
+              return ffma2(top, ly0p, fmul2(bot, ly1p));
             };
             float2 lo2 = lerp2(make_float2(v00.x, v00.y), make_float2(v01.x, v01.y), make_float2(v10.x, v10.y), make_float2(v11.x, v11.y));
             float2 hi2 = lerp2(make_float2(v00.z, v00.w), make_float2(v01.z, v01.w), make_float2(v10.z, v10.w), make_float2(v11.z, v11.w));
             if (pb) {
               const float4 c4 = __ldg(pb + f4);
-              lo2 = __fadd2_rn(lo2, make_float2(c4.x, c4.y));
-              hi2 = __fadd2_rn(hi2, make_float2(c4.z, c4.w));
+              lo2 = fadd2(lo2, make_float2(c4.x, c4.y));
+              hi2 = fadd2(hi2, make_float2(c4.z, c4.w));
             }
             y[u * 4 + 0] = lo2.x; y[u * 4 + 1] = lo2.y; y[u * 4 + 2] = hi2.x; y[u * 4 + 3] = hi2.y;
           }
 #pragma unroll
           for (int j = 0; j < 8; ++j) y[j] = valid ? fmaxf(y[j], 0.f) : 0.f;
-          store_a8<kPasses == 3>(m.a_hi + h * kAChunk, m.a_lo + h * kAChunk, row, g * 8, y);
+          store_a8<kPasses == 3>(m.a_hi + h * kAChunk, m.a_lo + h * kAChunk, row, gi * 8, y);
         }
         fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(m.bars + A1_FULL);
+        named_barrier(2 + g, 128);
       }
-      // ---- phase 1: y = lrelu(BN(x)*(1+gamma)+beta), chunks 0,1 from half R, chunks 2,3 from half R'
+      int frow[2];
+      bool fvalid[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        frow[i] = g * 64 + frag_row(t, i);
+        fvalid[i] = ti * 128 + frow[i] < a.HW;
+      }
 #pragma unroll 1
-      for (int kc = 0; kc < 4; ++kc, ++acnt) {
-        const int c0 = kc * 64 + h * 32;
-        const uint32_t col = (kc >> 1) * 256 + (kc & 1) * 128 + h * 32;      // index into the bias table
-        const uint32_t tcol = (kc < 2 ? R : Rp) + (kc & 1) * 128 + h * 32;   // TMEM column
-        float cur[32];
-        take_x_pair(m, xg, h, row, lane, cur);
-        if (kc == 0) {   // gamma/beta of channels 0..127 ready; A1 may be overwritten only after BOTH gamma/beta GEMMs
-          mbar_wait_sleep(m.bars + G1A_FULL, it & 1);
-          mbar_wait_sleep(m.bars + G1B_FULL, it & 1);
-          tc_fence_after();
-        }
-        uint32_t gr[32], br[32];
-        tmem_ld32(tmem + (static_cast<uint32_t>(q * 32) << 16) + tcol, gr);
-        tmem_ld32(tmem + (static_cast<uint32_t>(q * 32) << 16) + tcol + 64, br);
-        tmem_ld_wait();
-        const uint32_t slot = acnt & 1;
-        // chunks 0,1 overwrite A1 (free: G1B_FULL); chunks 2,3 wait for the conv to have consumed chunks 0,1
-        mbar_wait_sleep(m.bars + A_EMPTY + slot, ((acnt >> 1) & 1) ^ 1);
+      for (int kc = 0; kc < 4; ++kc) {
+        // ---- [gamma | beta] of channels 64kc.. (waits for the previous conv chunk too: the y chunk is free afterwards)
+        for (int k = 0; k < 2; ++k)
+          pipe_chunk<128, kPasses>(m, p, e, smem_u32(m.a_hi + k * kAChunk) + g * 64 * 128, smem_u32(m.a_lo + k * kAChunk) + g * 64 * 128,
+                                   k > 0, t);
+        pipe_drain<128>(m, p, e, t);
+        // ---- y = lrelu(BN(x)*(1+gamma)+beta) straight from the fragments; x from the chunk's two activation slices
+        const uint32_t s0 = ring_take(m, xg, 0, m.xs_n), s1 = ring_take(m, xg + 1, 0, m.xs_n);
+        xg += 2;
+        const float* xs0 = m.x_st + s0 * (kXSlice / 4);
+        const float* xs1 = m.x_st + s1 * (kXSlice / 4);
+        const int col = (kc >> 1) * 256 + (kc & 1) * 128;       // this chunk's gamma columns in the bias table
 #pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          float y[8], bg[8], bb[8], t1[8], t0[8];
-          lds8(tbgb + (col + g * 8) * 4, bg);
-          lds8(tbgb + (col + 64 + g * 8) * 4, bb);
-          lds8(tg1 + (c0 + g * 8) * 4, t1);
-          lds8(tg0 + (c0 + g * 8) * 4, t0);
+        for (int j = 0; j < 8; ++j) {
+          const int c = frag_col(t, j, 0), ch = kc * 64 + c;
+          const float* xs = j < 4 ? xs0 : xs1;
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const int jj = g * 8 + j;
-            const float gam = __uint_as_float(gr[jj]) + bg[j];        // 1 + gamma
-            const float bet = __uint_as_float(br[jj]) + bb[j];        // beta
-            const float xn = fmaf(cur[jj], t1[j], t0[j]);
-            const float v = fmaf(xn, gam, bet);
-            y[j] = valid ? fmaxf(v, 0.2f * v) : 0.f;
+          for (int i = 0; i < 2; ++i) {
+            float y2[2];
+#pragma unroll
+            for (int u = 0; u < 2; ++u) {
+              const float gam = e[4 * j + 2 * i + u] + m.tab_bgb[col + c + u];               // 1 + gamma
+              const float bet = e[4 * (j + 8) + 2 * i + u] + m.tab_bgb[col + 64 + c + u];    // beta
+              const float xn = fmaf(xs[((c + u) & 31) * 128 + frow[i]], m.tab_g1[ch + u], m.tab_g0[ch + u]);
+              const float v = fmaf(xn, gam, bet);
+              y2[u] = fvalid[i] ? fmaxf(v, 0.2f * v) : 0.f;
+            }
+            uint32_t hb, lb;
+            split_bf16x2(y2[0], y2[1], hb, lb);
+            const uint32_t off = sw128_offset(frow[i], c);
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(smem_u32(y_hi) + off), "r"(hb));
+            if (kPasses == 3) asm volatile("st.shared.b32 [%0], %1;" ::"r"(smem_u32(y_lo) + off), "r"(lb));
           }
-          store_a8<kPasses == 3>(m.a_hi + slot * kAChunk, m.a_lo + slot * kAChunk, row, h * 32 + g * 8, y);
         }
-        tc_fence_before();
+        ring_release(m, s0);
+        ring_release(m, s1);
         fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(m.bars + A_FULL + slot);
+        named_barrier(2 + g, 128);
+        pipe_chunk<256, kPasses>(m, p, d, smem_u32(y_hi) + g * 64 * 128, smem_u32(y_lo) + g * 64 * 128, kc > 0, t);
       }
+      pipe_drain<256>(m, p, d, t);
+      epilogue_fwd_any(a, m, d, b, ti, tm.T, g, t, sg);
     }
-  } else if (warp < 12) {
-    epilogue_team_loop(a, m, tm, tmem, warp - 8, lane);
-  } else if (warp == 12) {
-    {
-      const bool leader = elect_one_sync();
-      const uint32_t idesc = umma_idesc_bf16(128, 256);
-      MmaPipe p;
-      uint32_t acnt = 0;
-      for (int it = 0; it < tm.count; ++it) {
-        const uint32_t R = (it & 1) * 256, Rp = 256 - R;
-        auto a1_hi = [&](int kc) { return smem_u32(m.a_hi + kc * kAChunk); };
-        auto a1_lo = [&](int kc) { return smem_u32(m.a_lo + kc * kAChunk); };
-        mbar_wait_sleep(m.bars + A1_FULL, it & 1);
-        tc_fence_after();
-        // gamma|beta of channels 0..127 -> half R: free since the previous tile read its chunks 2,3 from it
-        // (that tile's A_FULL arrivals for chunks 2,3 precede this tile's A1_FULL)
-        for (int kc = 0; kc < 2; ++kc) mma_chunk<kPasses>(m, p, leader, tmem + R, a1_hi(kc), a1_lo(kc), idesc, kc > 0);
-        umma_commit_if(leader, m.bars + G1A_FULL);
-        // gamma|beta of channels 128..255 -> half R': holds the previous tile's conv accumulator until drained
-        if (it > 0) mbar_wait_sleep(m.bars + ACC_EMPTY + ((it - 1) & 1), ((it - 1) >> 1) & 1);
-        tc_fence_after();
-        for (int kc = 0; kc < 2; ++kc) mma_chunk<kPasses>(m, p, leader, tmem + Rp, a1_hi(kc), a1_lo(kc), idesc, kc > 0);
-        umma_commit_if(leader, m.bars + G1B_FULL);
-        // conv -> half R: y chunks 0 and 1 must BOTH exist first (their gamma/beta live in R)
-        const uint32_t ph0 = (acnt >> 1) & 1;
-        mbar_wait_sleep(m.bars + A_FULL + 0, ph0);
-        mbar_wait_sleep(m.bars + A_FULL + 1, ph0);
-        tc_fence_after();
-        for (int kc = 0; kc < 4; ++kc, ++acnt) {
-          const uint32_t slot = acnt & 1;
-          if (kc >= 2) {
-            mbar_wait_sleep(m.bars + A_FULL + slot, (acnt >> 1) & 1);
-            tc_fence_after();
-          }
-          mma_chunk<kPasses>(m, p, leader, tmem + R, smem_u32(m.a_hi + slot * kAChunk), smem_u32(m.a_lo + slot * kAChunk), idesc, kc > 0);
-          umma_commit_if(leader, m.bars + A_EMPTY + slot);
-        }
-        umma_commit_if(leader, m.bars + ACC_FULL + (it & 1));
-      }
-    }
-  } else if (warp == 13) {
-    if (lane == 0) {
-      // gamma/beta image: [2 nblocks][2 kchunks][hi,lo] = 8 stages, then the conv image: 8 stages
-      const uint8_t* imgs[2] = {a.wgb, a.wimg};
-      const int ns[2] = {8, 8};
-      weight_producer_loop<kPasses>(m, imgs, ns, 2, tm.count);
-    }
-  } else if (warp == 14) {
-    if (lane == 0) x_producer_loop(a, m, tm);
+    flush_fwd_stats(a, m);
   } else {
-    if (lane == 0) skip_producer_loop(a, m, tm);
+    regs_dec<kProducerRegs>();
+    if (lane == 0) {
+      if (warp == 8) pixel_weight_producer_loop<kPasses>(a, m, tm.count);
+      else if (warp == 9) x_producer_loop(a, m, tm);
+      else if (warp == 10) skip_producer_loop(a, m, tm);
+    }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 12) tmem_dealloc<512>(tmem);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1067,16 +927,16 @@ int hg_spade_conv(const float* x, long x_bstride, const float* mod, const float*
   const int tiles = B * ((Hg * Wg + 127) / 128);
   const int grid = tiles < hg::num_sms() ? tiles : hg::num_sms();
   auto st = static_cast<cudaStream_t>(stream);
-#define HG_LAUNCH(KERNEL, THREADS)                                                                                \
+#define HG_LAUNCH(KERNEL, SMEM)                                                                                   \
   do {                                                                                                            \
-    cudaError_t e = cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, hg::kSynSmemBytes); \
+    cudaError_t e = cudaFuncSetAttribute(KERNEL, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);               \
     if (e != cudaSuccess) { hg::set_error("hg_spade_conv: smem opt-in failed: %s", cudaGetErrorString(e)); return 2; } \
-    KERNEL<<<grid, THREADS, hg::kSynSmemBytes, st>>>(a);                                                          \
+    KERNEL<<<grid, hg::kSynThreads, SMEM, st>>>(a);                                                               \
   } while (0)
   if (mod) {
-    if (passes == 3) HG_LAUNCH((hg::spade_const_kernel<3, false>), hg::kSynThreads); else HG_LAUNCH((hg::spade_const_kernel<1, false>), hg::kSynThreads);
+    if (passes == 3) HG_LAUNCH((hg::spade_const_kernel<3, false>), hg::kSynSmemBytes); else HG_LAUNCH((hg::spade_const_kernel<1, false>), hg::kSynSmemBytes);
   } else {
-    if (passes == 3) HG_LAUNCH(hg::spade_pixel_kernel<3>, hg::kSynThreads); else HG_LAUNCH(hg::spade_pixel_kernel<1>, hg::kSynThreads);
+    if (passes == 3) HG_LAUNCH(hg::spade_pixel_kernel<3>, hg::kPixSmemBytes); else HG_LAUNCH(hg::spade_pixel_kernel<1>, hg::kPixSmemBytes);
   }
 #undef HG_LAUNCH
   return hg::check_launch("hg_spade_conv");

@@ -4,9 +4,9 @@
 // With the folded forward  pre = x*g1[b,c] + g0[b,c],  y = lrelu_0.2(pre),  out = W y + bias (+ skip) the
 // gradients split into three streaming kernels over the tile-blocked activations [B, T, C=256, 128]:
 //
-//   hg_spade_bwd_dgrad   (csrc/synth.cu, tcgen05)   dpre = (W^T dout) * lrelu'(pre);  S1[b,c] = sum dpre,
+//   hg_spade_bwd_dgrad   (csrc/synth.cu, wgmma)     dpre = (W^T dout) * lrelu'(pre);  S1[b,c] = sum dpre,
 //                                                   S2[b,c] = sum dpre*x
-//   hg_spade_bwd_wgrad   (here, tcgen05)            dW[co,ci] = sum_{b,p} dout[b,co,p] * y[b,ci,p]  (y recomputed),
+//   hg_spade_bwd_wgrad   (here, wgmma)              dW[co,ci] = sum_{b,p} dout[b,co,p] * y[b,ci,p]  (y recomputed),
 //                                                   dbias[co] = sum dout
 //   hg_spade_bwd_combine (here, streaming)          dL/dx = dpre*g1[b,c] + a[c] + k[c]*x  (+ skip gradient)
 //                                                   (+ W_rgb^T drgb), and the ToRGB weight gradient
@@ -16,16 +16,16 @@
 //
 // wgrad layout.  Both operands of dW = dout . y^T are K-major in the blocked layout as stored (K = pixels, 128
 // contiguous per channel row), so the operand warps only convert rows (coalesced 256 B row segments -> bf16 hi/lo
-// SW128 images); per-row constants (g1, g0) instead of per-column ones.  The [256 x 256] fp32 accumulator fills
-// the whole TMEM (two M=128 halves x 256 columns) for the CTA's lifetime and is written once, as a per-CTA
-// partial, then reduced deterministically by `wgrad_reduce_kernel`.
+// SW128 images); per-row constants (g1, g0) instead of per-column ones.  A CTA owns one 128-column half of dW (blockIdx.y):
+// its four warpgroups each keep a [64 x 128] fp32 accumulator (output channels 64w..64w+63) in registers for the CTA's
+// lifetime, written once as a per-CTA partial, then reduced deterministically by `wgrad_reduce_kernel`.
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace hg {
 
 constexpr int kWC = 256;
-constexpr int kWgThreads = 512;                 // 16 operand warps; warp 0 also issues the MMAs (one elected lane)
+constexpr int kWgThreads = 512;                 // 16 operand warps = four warpgroups, each also issuing its wgmmas
 constexpr uint32_t kWgImg = 256 * 128;          // [256 rows x 64 px] bf16 = 32 KB
 // dout image (hi, lo) double-buffered, x image (hi, lo) single: 6 x 32 KB
 constexpr uint32_t kWgSmemBytes = 6 * kWgImg + 8 * 8 + 16 + 1024;
@@ -35,15 +35,13 @@ struct WgradArgs {
   const float* x;        // [B or 1,T,C,128]
   long x_bstride;
   const float* mod;      // [B,2,C] g1, g0
-  float* part_w;         // [grid, C, nq]
+  float* part_w;         // [grid, C, nq]: CTA (x, y) writes columns 128y..128y+127 of partial x
   float* part_b;         // [grid, C]
   int B, HW;
   int nq;                // rows (channels) of the second operand x: 256, or 128 (gamma/beta weight gradients)
   int act;               // y = 0: lrelu_0.2(x*g1+g0), 1: sin(x*g1+g0), 2: x (identity)
   const float* pscale;   // [B,C] per-(b,row) scale of dout, or null
 };
-
-enum { WG_FULL = 0, WG_EMPTY = 1, WG_DONE = 2 };
 
 // the renderer's sine (csrc/render.cu `sin_reduced`): Cody-Waite reduction by 2*pi + SFU
 __device__ __forceinline__ float wg_red(float t) {
@@ -55,13 +53,12 @@ __device__ __forceinline__ float wg_red(float t) {
 __device__ __forceinline__ float wg_sin(float t) { return __sinf(wg_red(t)); }
 __device__ __forceinline__ float wg_cos(float t) { return __cosf(wg_red(t)); }
 
-// Schedule (chunk c = 64 pixels of a tile; a thread owns 8 pixels of 4 rows per operand):
+// Schedule (chunk c = 64 pixels of a tile; a thread owns 8 pixels of 4 dout rows and 2 x rows):
 //     convert x(c) -> B image      needs MMA(c-1) done (single buffer)
-//     arrive FULL(c); lane 0 of warp 0 issues MMA(c) on (A[c&1], B)
+//     barrier; every warpgroup issues MMA(c) on (its 64 rows of A[c&1], B)
 //     convert dout(c+1) -> A[(c+1)&1]   while MMA(c) runs (that slot was read last by MMA(c-1))
 // and the global loads of chunk c+1 (x) / c+2 (dout) are issued as soon as their registers are free, so HBM latency is
-// hidden behind the conversions and the MMA wait.  (The first version had 8 operand warps, one image of each operand and
-// loaded x only after converting dout: ncu showed 29 % of the samples waiting for MMA(c-1) and 14 % on the exposed x loads.)
+// hidden behind the conversions and the MMA wait.
 template <int kPasses, int kAct>
 __global__ void __launch_bounds__(kWgThreads, 1) spade_wgrad_kernel(WgradArgs a) {
   extern __shared__ uint8_t smem_raw[];
@@ -69,35 +66,21 @@ __global__ void __launch_bounds__(kWgThreads, 1) spade_wgrad_kernel(WgradArgs a)
   uint8_t* a_img = s;                      // [slot][hi, lo]
   uint8_t* b_hi = s + 4 * kWgImg;
   uint8_t* b_lo = s + 5 * kWgImg;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(s + 6 * kWgImg);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 8);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  if (threadIdx.x == 0) {
-    mbar_init(bars + WG_FULL, 16);
-    mbar_init(bars + WG_EMPTY, 1);
-    mbar_init(bars + WG_DONE, 1);
-    fence_mbar_init();
-  }
-  if (warp == 0) tmem_alloc<512>(tmem_slot);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_slot;
+  const int warp = threadIdx.x >> 5;
+  const int wg = warp >> 2, t128 = threadIdx.x & 127;     // warpgroup wg: output channels 64wg..64wg+63
+  const int ch = blockIdx.y;                              // columns (x channels) 128ch..128ch+127
 
   const int T = (a.HW + 127) / 128;
   const int total = a.B * T;
   const int count = (total - static_cast<int>(blockIdx.x) + static_cast<int>(gridDim.x) - 1) / static_cast<int>(gridDim.x);
   const int nchunks = 2 * count;
   const int nq = a.nq, HW = a.HW;
-  const int nst = nq >> 6;                    // row steps of the x operand: 4 (256 rows) or 2 (128)
-  const bool leader = warp == 0 && elect_one_sync();     // warp-uniform condition first: only warp 0 executes the elect
-  const uint32_t idesc = umma_idesc_bf16(128, nq);
 
   const int sub = threadIdx.x & 7;            // which 8-pixel group of the 64-pixel chunk
   const int rsub = threadIdx.x >> 3;          // 0..63: row within a 64-row step
   float bsum[4] = {0.f, 0.f, 0.f, 0.f};
-  float4 va[8], vb[8];
+  float4 va[8], vb[4];
+  float d[64];
 
   // chunk c -> sample, tile, first pixel of this thread, pixels of the image left from there
   auto locate = [&](int c, int& b, int& ti, int& p0, int& nvalid) {
@@ -121,14 +104,12 @@ __global__ void __launch_bounds__(kWgThreads, 1) spade_wgrad_kernel(WgradArgs a)
   auto load_x = [&](int c) {
     int b, ti, p0, nv;
     locate(c, b, ti, p0, nv);
-    const float* base = a.x + static_cast<long>(b) * a.x_bstride + static_cast<long>(ti) * nq * 128 + rsub * 128 + p0;
+    const float* base = a.x + static_cast<long>(b) * a.x_bstride + (static_cast<long>(ti) * nq + ch * 128 + rsub) * 128 + p0;
 #pragma unroll
-    for (int st = 0; st < 4; ++st) {
-      if (st < nst) {
-        const float4* src = reinterpret_cast<const float4*>(base + st * 64 * 128);
-        vb[2 * st] = __ldcs(src);
-        vb[2 * st + 1] = __ldcs(src + 1);
-      }
+    for (int st = 0; st < 2; ++st) {
+      const float4* src = reinterpret_cast<const float4*>(base + st * 64 * 128);
+      vb[2 * st] = __ldcs(src);
+      vb[2 * st + 1] = __ldcs(src + 1);
     }
   };
   auto convert_d = [&](int c) {      // dout rows of chunk c -> A[c & 1]; bias partial sums
@@ -154,13 +135,13 @@ __global__ void __launch_bounds__(kWgThreads, 1) spade_wgrad_kernel(WgradArgs a)
       store_a8<kPasses == 3>(hi, lo, row, sub * 8, y);
     }
   };
-  auto convert_x = [&](int c) {      // x rows of chunk c -> act(x*g1 + g0) -> B
+  auto convert_x = [&](int c) {      // x rows 128ch.. of chunk c -> act(x*g1 + g0) -> B rows 0..127
     int b, ti, p0, nvalid;
     locate(c, b, ti, p0, nvalid);
 #pragma unroll
-    for (int st = 0; st < 4; ++st) {
-      if (st < nst) {
-        const int row = st * 64 + rsub;
+    for (int st = 0; st < 2; ++st) {
+      {
+        const int row = ch * 128 + st * 64 + rsub;
         float g1 = 1.f, g0 = 0.f;               // no table: y = act(x)
         if (a.mod) {
           g1 = __ldg(a.mod + (static_cast<long>(b) * 2 + 0) * kWC + row);
@@ -175,12 +156,12 @@ __global__ void __launch_bounds__(kWgThreads, 1) spade_wgrad_kernel(WgradArgs a)
           const float2 g1p = make_float2(g1, g1), g0p = make_float2(g0, g0);
 #pragma unroll
           for (int j = 0; j < 8; j += 2) {
-            const float2 v = __ffma2_rn(make_float2(y[j], y[j + 1]), g1p, g0p);
+            const float2 v = ffma2(make_float2(y[j], y[j + 1]), g1p, g0p);
             if (kAct == 2) {
               y[j] = v.x;
               y[j + 1] = v.y;
             } else {
-              const float2 sv = __fmul2_rn(v, make_float2(0.2f, 0.2f));
+              const float2 sv = fmul2(v, make_float2(0.2f, 0.2f));
               y[j] = fmaxf(v.x, sv.x);
               y[j + 1] = fmaxf(v.y, sv.y);
             }
@@ -190,7 +171,7 @@ __global__ void __launch_bounds__(kWgThreads, 1) spade_wgrad_kernel(WgradArgs a)
 #pragma unroll
           for (int j = 0; j < 8; ++j) y[j] = j < nvalid ? y[j] : 0.f;
         }
-        store_a8<kPasses == 3>(b_hi, b_lo, row, sub * 8, y);
+        store_a8<kPasses == 3>(b_hi, b_lo, st * 64 + rsub, sub * 8, y);
       }
     }
   };
@@ -201,70 +182,54 @@ __global__ void __launch_bounds__(kWgThreads, 1) spade_wgrad_kernel(WgradArgs a)
     convert_d(0);
     if (nchunks > 1) load_d(1);
     for (int c = 0; c < nchunks; ++c) {
-      if (c > 0) mbar_wait_sleep(bars + WG_EMPTY, (c - 1) & 1);      // MMA(c-1) done: B and A[(c-1)&1] are free
+      if (c > 0) {      // MMA(c-1) done in every warpgroup: B and A[(c-1)&1] are free
+        wgmma_wait<0>();
+        acc_fence(d);
+        __syncthreads();
+      }
       convert_x(c);
       if (c + 1 < nchunks) load_x(c + 1);
       fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bars + WG_FULL);
-      if (warp == 0) {      // the whole warp waits; its elected lane issues (convergent code: descriptors in uniform registers)
-        mbar_wait_sleep(bars + WG_FULL, c & 1);
-        tc_fence_after();
-        const uint32_t ah0 = smem_u32(a_img + (c & 1) * 2 * kWgImg), al0 = ah0 + kWgImg;
-#pragma unroll
-        for (uint32_t mh = 0; mh < 2; ++mh) {
-          const uint32_t d = tmem + mh * 256;
-          const uint32_t ah = ah0 + mh * (kWgImg / 2), al = al0 + mh * (kWgImg / 2);
-          umma_k64_if(leader, d, ah, smem_u32(b_hi), idesc, c > 0);
-          if (kPasses == 3) {
-            umma_k64_if(leader, d, al, smem_u32(b_hi), idesc, true);
-            umma_k64_if(leader, d, ah, smem_u32(b_lo), idesc, true);
-          }
-        }
-        umma_commit_if(leader, bars + WG_EMPTY);
-        if (c + 1 == nchunks) umma_commit_if(leader, bars + WG_DONE);
+      __syncthreads();
+      const uint32_t ah = smem_u32(a_img + (c & 1) * 2 * kWgImg) + wg * 64 * 128, al = ah + kWgImg;
+      acc_fence(d);
+      wgmma_fence();
+      wg_k64<128>(d, ah, smem_u32(b_hi), c > 0);
+      if (kPasses == 3) {
+        wg_k64<128>(d, al, smem_u32(b_hi), true);
+        wg_k64<128>(d, ah, smem_u32(b_lo), true);
       }
+      wgmma_commit();
       if (c + 1 < nchunks) {
         convert_d(c + 1);
         if (c + 2 < nchunks) load_d(c + 2);
       }
     }
+    wgmma_wait<0>();
+    acc_fence(d);
   }
-  // bias-gradient partials: row (st*64 + rsub) is shared by the 8 `sub` lanes
+  // bias-gradient partials (CTAs of column half 0): row (st*64 + rsub) is shared by the 8 `sub` lanes
 #pragma unroll
   for (int st = 0; st < 4; ++st) {
     float v = bsum[st];
     v += __shfl_xor_sync(0xffffffffu, v, 1);
     v += __shfl_xor_sync(0xffffffffu, v, 2);
     v += __shfl_xor_sync(0xffffffffu, v, 4);
-    if (sub == 0) a.part_b[static_cast<long>(blockIdx.x) * kWC + st * 64 + rsub] = v;
+    if (sub == 0 && ch == 0) a.part_b[static_cast<long>(blockIdx.x) * kWC + st * 64 + rsub] = v;
   }
-  // ---- drain: warps 0-3 own TMEM lanes 32w..32w+31 (co within the half), 2 x 256 columns (ci)
-  if (warp < 4) {
-    float* dst = a.part_w + static_cast<long>(blockIdx.x) * kWC * a.nq;
-    if (count > 0) {
-      mbar_wait_sleep(bars + WG_DONE, 0);
-      tc_fence_after();
-      for (int mh = 0; mh < 2; ++mh) {
-        const int co = mh * 128 + warp * 32 + lane;
-        for (int cg = 0; cg < (a.nq >> 5); ++cg) {
-          uint32_t raw[32];
-          tmem_ld32(tmem + mh * 256 + (static_cast<uint32_t>(warp * 32) << 16) + cg * 32, raw);
-          tmem_ld_wait();
-          float4* o = reinterpret_cast<float4*>(dst + static_cast<long>(co) * a.nq + cg * 32);
+  // ---- drain: output channel 64wg + frag_row, x channel 128ch + frag_col
+  float* dst = a.part_w + static_cast<long>(blockIdx.x) * kWC * a.nq + ch * 128;
+  if (count > 0) {
 #pragma unroll
-          for (int j = 0; j < 8; ++j)
-            o[j] = make_float4(__uint_as_float(raw[4 * j]), __uint_as_float(raw[4 * j + 1]), __uint_as_float(raw[4 * j + 2]),
-                               __uint_as_float(raw[4 * j + 3]));
-        }
-      }
-    } else {
-      for (int i = threadIdx.x; i < kWC * a.nq; i += 128) dst[i] = 0.f;
+    for (int i = 0; i < 2; ++i) {
+      const int co = wg * 64 + frag_row(t128, i);
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+        *reinterpret_cast<float2*>(dst + static_cast<long>(co) * a.nq + frag_col(t128, j, 0)) = make_float2(d[4 * j + 2 * i], d[4 * j + 2 * i + 1]);
     }
+  } else {
+    for (int i = threadIdx.x; i < kWC * 128; i += kWgThreads) dst[static_cast<long>(i >> 7) * a.nq + (i & 127)] = 0.f;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc<512>(tmem);
 }
 
 // dW[i] = sum over CTAs of part[cta][i] (fp64 accumulation, fixed order -> deterministic), likewise the bias.
@@ -465,16 +430,16 @@ __global__ void __launch_bounds__(128) a1_gather_kernel(const float* __restrict_
     // are bit-identical to what the forward multiplied with
     const float2 lx0p = make_float2(lx0, lx0), lx1p = make_float2(lx1, lx1), ly0p = make_float2(ly0, ly0), ly1p = make_float2(ly1, ly1);
     auto lerp2 = [&](float2 a, float2 b, float2 c, float2 d) {
-      const float2 top = __ffma2_rn(b, lx1p, __fmul2_rn(a, lx0p));
-      const float2 bot = __ffma2_rn(d, lx1p, __fmul2_rn(c, lx0p));
-      return __ffma2_rn(top, ly0p, __fmul2_rn(bot, ly1p));
+      const float2 top = ffma2(b, lx1p, fmul2(a, lx0p));
+      const float2 bot = ffma2(d, lx1p, fmul2(c, lx0p));
+      return ffma2(top, ly0p, fmul2(bot, ly1p));
     };
     float2 lo2 = lerp2(make_float2(v00.x, v00.y), make_float2(v01.x, v01.y), make_float2(v10.x, v10.y), make_float2(v11.x, v11.y));
     float2 hi2 = lerp2(make_float2(v00.z, v00.w), make_float2(v01.z, v01.w), make_float2(v10.z, v10.w), make_float2(v11.z, v11.w));
     if (pb) {
       const float4 c4 = __ldg(pb + f4);
-      lo2 = __fadd2_rn(lo2, make_float2(c4.x, c4.y));
-      hi2 = __fadd2_rn(hi2, make_float2(c4.z, c4.w));
+      lo2 = fadd2(lo2, make_float2(c4.x, c4.y));
+      hi2 = fadd2(hi2, make_float2(c4.z, c4.w));
     }
     const float4 y = make_float4(lo2.x, lo2.y, hi2.x, hi2.y);
     dst[(f4 * 4 + 0) * 128] = valid ? fmaxf(y.x, 0.f) : 0.f;
@@ -673,7 +638,7 @@ int hg_act_wgrad_blocked(const float* dout, const float* pscale, const float* x,
 #define HG_WG_LAUNCH(P, A)                                                                                              \
   do {                                                                                                                  \
     e = cudaFuncSetAttribute(hg::spade_wgrad_kernel<P, A>, cudaFuncAttributeMaxDynamicSharedMemorySize, hg::kWgSmemBytes); \
-    if (e == cudaSuccess) hg::spade_wgrad_kernel<P, A><<<grid, hg::kWgThreads, hg::kWgSmemBytes, st>>>(a);              \
+    if (e == cudaSuccess) hg::spade_wgrad_kernel<P, A><<<dim3(grid, Cx / 128), hg::kWgThreads, hg::kWgSmemBytes, st>>>(a); \
   } while (0)
   if (passes == 3) {
     if (act == 0) HG_WG_LAUNCH(3, 0); else if (act == 1) HG_WG_LAUNCH(3, 1); else HG_WG_LAUNCH(3, 2);

@@ -81,7 +81,7 @@ class UNetDiscriminator(nn.Module):
         from . import discriminator_ops
         from .generator import _precision_passes
         if torch.is_grad_enabled() and (images.requires_grad or any(p.requires_grad for p in self.parameters())):
-            # discriminator / generator step of the trainer: the autograd graph over the sm_100a primitives
+            # discriminator / generator step of the trainer: the autograd graph over the sm_90a primitives
             from . import discriminator_train
             return discriminator_train.discriminator_forward_train(self, images, passes=_precision_passes(kwargs),
                                                                    masks=kwargs.get("hg_record_masks"))

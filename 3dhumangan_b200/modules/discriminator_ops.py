@@ -1,4 +1,4 @@
-"""Host-side schedule of the U-Net discriminator on the sm_100a convolution kernels (csrc/dconv.cu).
+"""Host-side schedule of the U-Net discriminator on the sm_90a convolution kernels (csrc/dconv.cu).
 
 Mirrors `UNetDiscriminator.forward` / `ResBlock.forward` (lib/discriminators/unet_discriminators.py:47-72,
 125-160).  Per ResBlock: two implicit-GEMM 3x3 convolutions with LeakyReLU / nearest up-sample / channel

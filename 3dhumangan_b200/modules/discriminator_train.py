@@ -1,4 +1,4 @@
-"""Training-mode U-Net discriminator: autograd graph over the sm_100a primitives.
+"""Training-mode U-Net discriminator: autograd graph over the sm_90a primitives.
 
 The inference path (`discriminator_ops.discriminator_forward`) folds LeakyReLU / up-sample / concat / residual into
 the convolution kernel.  For training the same network is an ordinary autograd graph whose nodes are this library's
@@ -6,7 +6,7 @@ ops, so that first-order gradients w.r.t. images (generator step) and parameters
 `loss.backward()`:
 
     convolution      `Conv2dSame`  forward `hg_conv2d`, data gradient `hg_conv2d` with the rotated / transposed filter,
-                                   weight gradient `ConvWgrad` = `hg_conv2d_wgrad_taps` (tcgen05); both backward nodes
+                                   weight gradient `ConvWgrad` = `hg_conv2d_wgrad_taps` (wgmma); both backward nodes
                                    are themselves differentiable (R1 double backward, phase_trainer.py:259-294)
     LeakyReLU        `ops.bias_act` (hg_bias_act / hg_bias_act_grad)
     avg-pool / nearest up-sample   `ops.upfirdn2d` with a 2x2 box filter (its backward is another upfirdn pass)

@@ -9,9 +9,9 @@ reference's ~150 ATen launches:
 
     hg_geo_features   rays + jitter + camera transform + exact nearest-vertex search + 31-d feature
     hg_render_mlp     FiLM-SIREN MLP + volume integration, one kernel, only [rays, 260] leaves the SM
-    hg_spade_conv x18 SPADE half-blocks with BatchNorm / modulation / ToRGB fused around tcgen05 GEMMs
+    hg_spade_conv x18 SPADE half-blocks with BatchNorm / modulation / ToRGB fused around wgmma GEMMs
 
-There is no CPU or eager-PyTorch fallback: without a CUDA device and lib3dhg_sm100a.so the
+There is no CPU or eager-PyTorch fallback: without a CUDA device and lib3dhg_sm90a.so the
 forward raises RuntimeError.  With autograd enabled on parameters that require grad, `forward` runs the
 training kernels (modules/render_train.py, modules/synthesis_train.py) and its outputs are differentiable.
 """
@@ -63,7 +63,7 @@ def _kaiming_leaky_(w, a=0.2):
 
 class MappingNetwork(nn.Module):
     """z -> (freq, phase) for the SIREN (lib/components/mapping_networks.py:13-41).  The four dense layers run on the
-    tcgen05 GEMM (`ops.dense`, fp32 via the bf16x3 split), LeakyReLU on `ops.bias_act`; the `nn.Linear` /
+    wgmma GEMM (`ops.dense`, fp32 via the bf16x3 split), LeakyReLU on `ops.bias_act`; the `nn.Linear` /
     `nn.LeakyReLU` children only hold the parameters under the reference's state_dict names."""
 
     def __init__(self, latent_dim, map_hidden_dim, map_output_dim):
@@ -93,7 +93,7 @@ class MappingNetwork(nn.Module):
 
 
 class FullyConnectedLayer(nn.Module):
-    """StyleGAN-style equalised-lr dense layer (mapping_networks.py:92-121): the product on the tcgen05 GEMM with the
+    """StyleGAN-style equalised-lr dense layer (mapping_networks.py:92-121): the product on the wgmma GEMM with the
     weight gain folded into the operand packing (`ops.dense`), bias + activation through the `bias_act` kernel."""
 
     def __init__(self, in_features, out_features, bias=True, activation="linear", lr_multiplier=1, bias_init=0):

@@ -2,7 +2,7 @@
 
 The module owns the parameters under the reference's names (`first_layer_coord.layer.*`,
 `first_layer_mod.layer.*`, `network.{i}.layer.*`, `sigma_layer.*`, `color_layer_sine.layer.*`,
-`color_layer_linear.*`, `feature_layer_linear.*`) and evaluates the MLP with the fused sm_100a
+`color_layer_linear.*`, `feature_layer_linear.*`) and evaluates the MLP with the fused sm_90a
 kernel.  Inside `Map3DGenerator` the MLP never runs on its own (it is fused with the ray
 integration in `hg_render_mlp`); `forward()` is provided for callers that want raw
 per-point outputs and uses the same kernel with one sample per "ray".

@@ -14,18 +14,22 @@ from .. import abi
 
 def pack_render_weights(P, prefix="neural_field.", geo_dim=31):
     """Concatenate the packed bf16 hi/lo operand images of the MLP in the kernel's schedule order
-    (render.cu): W01 = [coord | geo] block matrix, network.0 (K=512), network.1-3, color[:, 3:], feature."""
+    (render.cu): W01 = [coord | geo] block matrix, network.0 (K=512: the geometry half first), network.1-3, color[:, 3:],
+    feature."""
     g = lambda n: P[prefix + n]
     dev = g("network.0.layer.weight").device
     H = g("network.0.layer.weight").shape[0]
     if H != 256 or geo_dim + 3 > 36:
-        raise RuntimeError("hg3d: the sm_100a render kernel is built for hidden_dim == 256, geo_feature_dim <= 33")
+        raise RuntimeError("hg3d: the fused render kernel is built for hidden_dim == 256, geo_feature_dim <= 33")
     W01 = torch.zeros(2 * H, 3 + geo_dim, dtype=torch.float32, device=dev)
     W01[:H, :3] = g("first_layer_coord.layer.weight")
     W01[H:, 3:] = g("first_layer_mod.layer.weight")
     mats = [W01, g("network.0.layer.weight"), g("network.1.layer.weight"), g("network.2.layer.weight"),
             g("network.3.layer.weight"), g("color_layer_sine.layer.weight")[:, 3:], g("feature_layer_linear.weight")]
     imgs = [abi.pack_weight(m.float().contiguous() if m.stride(1) == 1 else m.float().contiguous(), Nb=256)[0] for m in mats]
+    # network.0 runs its geometry half (K chunks 4-7) first: the kernel computes g before a (render.cu, layer schedule)
+    half = imgs[1].numel() // 2
+    imgs[1] = torch.cat([imgs[1][half:], imgs[1][:half]])
     blob = torch.cat(imgs)
     assert blob.numel() == abi.lib().hg_render_weight_blob_bytes(), blob.numel()
     return blob

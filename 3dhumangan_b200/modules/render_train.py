@@ -1,5 +1,5 @@
 """Training-mode forward + backward of the FiLM-SIREN renderer (COORDCONCATSIREN.forward modulated.py:41-75 +
-vr.ray_integration volume_rendering.py:12-56) on the sm_100a kernels.
+vr.ray_integration volume_rendering.py:12-56) on the sm_90a kernels.
 
 The inference path is ONE fused kernel (csrc/render.cu) that keeps every activation on chip.  Training needs the
 pre-activations back, so here the MLP runs layer by layer over tile-blocked points [B, T, 256, 128] (the layout of the
@@ -51,7 +51,7 @@ def mlp_forward_train(P, freq, phase, rec, z_vals, noise, cfg, *, geo_dim=31, lo
     if cfg.get("last_back", False):
         raise RuntimeError("hg3d: last_back=True is an inference-only setting (eval_last_back); the training renderer does not build it")
     if g("network.0.layer.weight").shape[0] != H:
-        raise RuntimeError("hg3d: the sm_100a render kernels are built for hidden_dim == 256")
+        raise RuntimeError("hg3d: the sm_90a render kernels are built for hidden_dim == 256")
     f32 = dict(dtype=torch.float32, device=dev)
     kw = dict(B=B, Hg=1, Wg=N, passes=passes)
     pack = lambda w: abi.pack_weight(w.detach().float().contiguous(), Nb=256)[0]
@@ -230,7 +230,7 @@ def core_parameters(module):
 
 
 class GeneratorCore(torch.autograd.Function):
-    """(freq, phase, fixed style, *renderer and synthesis parameters) -> (rgbs, rgbs_render, depth) on the sm_100a kernels.
+    """(freq, phase, fixed style, *renderer and synthesis parameters) -> (rgbs, rgbs_render, depth) on the sm_90a kernels.
 
     EVERY parameter the kernels read is an input of this node and its gradient is RETURNED by `backward`, so the
     reference trainer's machinery sees them like any other autograd node's: `DistributedDataParallel` reducer hooks fire

@@ -5,7 +5,7 @@ Mirrors `SynthesisNetwork.forward` (lib/generators/map3d_generator.py:58-97) +
 `Map3DGenerator.forward` (:244-245), restructured around 18 fused half-block launches:
 
   * the up-sampled style map is never materialised: `mlp_shared` is applied to the render-resolution
-    feature map (one tcgen05 GEMM, `hg_linear`) and interpolated inside the half-block kernel;
+    feature map (one wgmma GEMM, `hg_linear`) and interpolated inside the half-block kernel;
   * half-blocks whose style is spatially constant get per-sample (1+gamma, beta) vectors and skip
     the gamma/beta GEMMs entirely;
   * BatchNorm statistics of every activation are produced by the epilogue of the kernel that
@@ -107,7 +107,7 @@ def synthesis_forward(params, feat_lr, fixed_style, cfg, *, training=True, passe
     Hg, Wg, Rh, Rw = cfg["gen_height"], cfg["gen_width"], cfg["render_height"], cfg["render_width"]
     C = cfg["hidden_dim"]
     if C != 256 or cfg["feature_dim"] != 256:
-        raise RuntimeError("hg3d: the sm_100a synthesis kernels are built for hidden_dim == feature_dim == 256")
+        raise RuntimeError("hg3d: the sm_90a synthesis kernels are built for hidden_dim == feature_dim == 256")
     HW = Hg * Wg
     nb = cfg["synthesis_blocks"]
     mode = cfg.get("map3d_mode", "isolated")

@@ -1,4 +1,4 @@
-"""Training-mode forward + backward of the SPADE synthesis network on the sm_100a kernels.
+"""Training-mode forward + backward of the SPADE synthesis network on the sm_90a kernels.
 
 Forward: the same 18 fused half-block launches as `synthesis_ops.synthesis_forward`, but every half-block
 input is kept (18 activations of B*HW*256 fp32 -- 2.1 GB each at the C2 workload; sized for 180 GB of HBM)
@@ -9,8 +9,8 @@ Backward (autograd through SynthesisNetwork.forward map3d_generator.py:58-97, SP
 map3d_layers.py:218-238, SPADE2d.forward :176-190, ToRGB :346-352, SynthesisInput :260-275), walking the
 half-blocks in reverse; per half-block
     hg_spade_bwd_combine  dL/dout   from the next half-block's dpre (+ skip gradient, + ToRGB^T drgb)
-    hg_spade_bwd_dgrad    dpre = (W^T dL/dout) * lrelu'(pre), S1 = sum dpre, S2 = sum dpre*x     (tcgen05)
-    hg_spade_bwd_wgrad    dW = dL/dout . y^T, dbias                                              (tcgen05)
+    hg_spade_bwd_dgrad    dpre = (W^T dL/dout) * lrelu'(pre), S1 = sum dpre, S2 = sum dpre*x     (wgmma)
+    hg_spade_bwd_wgrad    dW = dL/dout . y^T, dbias                                              (wgmma)
 and the small chains on the host side: d(g1,g0) = (S2,S1) -> BatchNorm weight/bias, gamma/beta MLP, fixed style,
 and -- through the leaves sum(x), sum(x^2) of the batch statistics -- the a[c] + k[c]*x term of dL/dx
 (SyncBatchNorm: those two leaf gradients are SUM-all-reduced, like the statistics themselves).
@@ -18,14 +18,14 @@ and -- through the leaves sum(x), sum(x^2) of the batch statistics -- the a[c] +
 Pixel-style half-blocks (per-pixel gamma/beta from the up-sampled render features; blocks in `mod_blocks`)
 keep the fused forward kernel and, in backward, REBUILD their per-pixel quantities instead of storing them:
     hg_spade_a1            A1 = relu(bilinear_up(P_lr) + c)                      [B,T,128,128]
-    hg_conv1x1_blocked x2  gam = Wg A1 + bg + 1,  bet = Wb A1 + bb               (tcgen05)
+    hg_conv1x1_blocked x2  gam = Wg A1 + bg + 1,  bet = Wb A1 + bb               (wgmma)
     hg_spade_pixel_pre     pre = (x*sc + sh)*gam + bet
 then the same dgrad / wgrad kernels run on `pre`, followed by
     hg_spade_pixel_mod_bwd dxn = dpre*gam, dgam = dpre*xn (+ the BatchNorm / bias sums)
-    hg_conv1x1_blocked_bwd dA1 = ([dgam | dpre] . [Wg | Wb]) * relu'(A1)        (tcgen05, K = 512, pixel-major out)
-    hg_wgrad_blocked   x2  dWg = dgam . A1^T,  dWb = dpre . A1^T                 (tcgen05)
+    hg_conv1x1_blocked_bwd dA1 = ([dgam | dpre] . [Wg | Wb]) * relu'(A1)        (wgmma, K = 512, pixel-major out)
+    hg_wgrad_blocked   x2  dWg = dgam . A1^T,  dWb = dpre . A1^T                 (wgmma)
     hg_bilinear_adjoint    dP_lr (render resolution)
-and once, at the end, d(feature maps) = dP_lr . W_shared (tcgen05 `hg_linear`) and dW_shared = dP_lr^T . features
+and once, at the end, d(feature maps) = dP_lr . W_shared (wgmma `hg_linear`) and dW_shared = dP_lr^T . features
 (a plain library GEMM through torch.matmul).
 """
 from __future__ import annotations
@@ -59,7 +59,7 @@ def synthesis_forward_train(params, feat_lr, fixed_style, cfg, *, passes=3, pref
     B = fixed_style.shape[0]
     Hg, Wg = cfg["gen_height"], cfg["gen_width"]
     if cfg["hidden_dim"] != C or cfg["feature_dim"] != C:
-        raise RuntimeError("hg3d: the sm_100a synthesis kernels are built for hidden_dim == feature_dim == 256")
+        raise RuntimeError("hg3d: the sm_90a synthesis kernels are built for hidden_dim == feature_dim == 256")
     HW = Hg * Wg
     T = (HW + 127) // 128
     nb = cfg["synthesis_blocks"]

@@ -1,8 +1,8 @@
 """Forward path for every hidden_dim / feature_dim <= 512 other than 256 -- the 256-pixel curriculum MAP3DBN (384,
 configs/map3d.py:3-95) and the released checkpoint's MAP3DBN512L (420, configs/map3d.py:194-290, doc/GET_STARTED.md:17-22).
 
-The fused kernels (csrc/render.cu, csrc/synth.cu's pixel-style kernel) are laid out for exactly 256 channels (TMEM plan,
-shared-memory budget).  Wider networks run on the library's GENERAL blocked-GEMM engine instead: every channel dimension is
+The fused kernels (csrc/render.cu, csrc/synth.cu's pixel-style kernel) are laid out for exactly 256 channels (register
+accumulators, shared-memory budget).  Wider networks run on the library's GENERAL blocked-GEMM engine instead: every channel dimension is
 zero-padded to 512 = two tile-blocked halves [B,T,256,128], and a 512 -> 512 layer is two launches of
 `hg_blocked_conv_wide` (K = 512 from two sources with a modulation table per source, N = 256 outputs each), with the same
 fused prologue (BatchNorm x SPADE modulation x LeakyReLU, or FiLM sine) and epilogue (bias, residual, ToRGB, next-layer

@@ -1,2 +1,2 @@
-"""`lib.components.ops` surface: bias_act and upfirdn2d on sm_100a (no 'ref' implementation, no JIT plugin)."""
+"""`lib.components.ops` surface: bias_act and upfirdn2d on sm_90a (no 'ref' implementation, no JIT plugin)."""
 from . import bias_act, upfirdn2d  # noqa: F401

@@ -2,7 +2,7 @@
 
 Same Python signature as the reference op.  The reference defaults to `impl='ref'` (plain torch
 ops) and its CUDA plugin cannot even be built (SURVEY.md fact 2); here there is exactly one
-implementation, the sm_100a kernels behind `hg_bias_act` / `hg_bias_act_grad`.
+implementation, the sm_90a kernels behind `hg_bias_act` / `hg_bias_act_grad`.
 
 Differentiable to second order like the reference's cached autograd classes (bias_act.py:124-207):
 the forward op saves y (or x for swish), its backward is itself an autograd op whose backward

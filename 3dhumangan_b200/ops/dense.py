@@ -1,4 +1,4 @@
-"""Dense layers of the two mapping networks on the tcgen05 GEMM (`hg_linear`), differentiable.
+"""Dense layers of the two mapping networks on the wgmma GEMM (`hg_linear`), differentiable.
 
     y = x @ (gain * W)^T + b          x [M,K], W [N,K], b [N]
 

@@ -1,4 +1,4 @@
-"""Loss + optimiser tail of the reference's training iteration on sm_100a kernels (csrc/trainer.cu; SURVEY.md 8f-1).
+"""Loss + optimiser tail of the reference's training iteration on sm_90a kernels (csrc/trainer.cu; SURVEY.md 8f-1).
 
   seg_ce_balanced   PhaseTrainer._calculate_segmentation_loss, mode 'cross_entropy_balanced' (phase_trainer.py:203-256):
                     label histogram -> per-class coefficients -> ONE pass over the logits that yields the loss and its gradient.

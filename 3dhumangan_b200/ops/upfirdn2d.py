@@ -1,6 +1,6 @@
 """upfirdn2d: pad / zero-insert up-sample / FIR / decimate  (reference: lib/components/ops/upfirdn2d.py:117-161,
 upfirdn2d.cu:29-375).  Same Python signatures (`upfirdn2d`, `setup_filter`, `filter2d`, `upsample2d`,
-`downsample2d`); one implementation, the sm_100a kernel behind `hg_upfirdn2d`.
+`downsample2d`); one implementation, the sm_90a kernel behind `hg_upfirdn2d`.
 
 Differentiable to any order in x: the adjoint of an up/FIR/down pass is the same kind of pass with up and
 down exchanged, the filter flipped and the padding mirrored (upfirdn2d.py:213-231 does the same), so the

@@ -11,7 +11,7 @@ does -- `DistributedDataParallel(find_unused_parameters=True, broadcast_buffers=
 `backward(retain_graph=True)`, `unscale_` / `clip_grad_norm_` / `scaler.step`, EMA over `parameters()`; (2) it is the
 G+D step that `bench.py` times (BASELINE.json's second metric).
 
-Everything between the inputs and the two losses runs on the sm_100a kernels (generator: fused inference kernels under
+Everything between the inputs and the two losses runs on the sm_90a kernels (generator: fused inference kernels under
 no_grad in the discriminator step, training kernels in the generator step; discriminator: the autograd graph of
 modules/discriminator_train.py).  Loss reduction, clipping, Adam and EMA are multi-tensor torch calls (SURVEY.md §8f-1).
 """
@@ -188,7 +188,7 @@ class Trainer:
     reference splats into every call."""
 
     def __init__(self, G, D, meta, *, amp=None, ddp=None, amp_dtype=torch.float16, ema_decay=0.999, fused=True):
-        """fused=True: the loss / clipping / Adam / EMA tail on the sm_100a kernels of csrc/trainer.cu (ops.trainer_ops);
+        """fused=True: the loss / clipping / Adam / EMA tail on the sm_90a kernels of csrc/trainer.cu (ops.trainer_ops);
         fused=False: the same steps as torch calls (F.cross_entropy, clip_grad_norm_, torch.optim.Adam, foreach lerp)."""
         import torch.distributed as dist
         self.meta = dict(meta)

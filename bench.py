@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Benchmark of the 3DHumanGAN generator hot path on B200 (and its CPU reference arm).
+"""Benchmark of the 3DHumanGAN generator hot path on H100 (and its CPU reference arm).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload C2|C2native|C5|tiny]
+                    [--dump-outputs DIR]
 
 One "step" = one `Map3DGenerator.forward` over one batch of synthetic latents + random SMPL-like poses
 (train-mode BatchNorm, as the reference's trainer runs the generator) at BASELINE.json configs[1]:
@@ -17,6 +18,11 @@ batch 8 per GPU, 512x512, render 96x96, 32 samples per ray.  Prints ONE JSON lin
 
 Multi-GPU (`torchrun ... bench.py --gpus N`): weak scaling, 8 images per rank, SyncBatchNorm statistics
 all-reduced over NCCL inside the forward (18 small all-reduces), no other data-path collective.
+
+--dump-outputs DIR writes what the timed path returned in its last timed step (rank 0) as DIR/<name>.npy (float32; the
+losses of a training iteration in float64), at most 64 MB in all: a larger output is replaced by a fixed, seeded sample of
+its elements.  Parameters, latents and poses are seeded, so two builds run with the same arguments can be compared output
+for output.
 """
 from __future__ import annotations
 
@@ -36,7 +42,10 @@ sys.path.insert(0, ROOT)
 
 METRIC = "images_per_sec_G_fwd_512x512"
 UNIT = "images/s"
-FALLBACK_PEAKS = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}
+# NVIDIA's H100 SXM data sheet (dense BF16, HBM3, for a card allowed 700 W): denominators of the roofline fractions, not
+# rates this benchmark has reached
+FALLBACK_PEAKS = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}
+DUMP_BYTES = 64 << 20
 
 
 _REAL_STDOUT = None
@@ -68,16 +77,19 @@ def peaks():
     return dict(FALLBACK_PEAKS, _source="fallback")
 
 
-def ncu_traffic(entry, workload):
-    """dram__bytes_read.sum + dram__bytes_write.sum per launch of the dominant kernel from the newest committed `ncu --set full`
-    capture of this workload (profiles/r2_ncu_traffic.json, written from tools/profile_r2.sh's export: the mean over the 18
-    half-block launches of one forward, all variants); null for workloads / kernels that were not captured.  (A profiler cannot
-    run inside the timed process; the capture is refreshed whenever the kernel changes.)"""
-    p = os.path.join(ROOT, "profiles", "r2_ncu_traffic.json")
-    if not os.path.exists(p):
-        return None
-    d = json.load(open(p)).get(entry, {}).get(workload)
-    return None if d is None else d["dram_bytes_per_launch_mean_of_18"]
+def dump_outputs(path, arrays):
+    """arrays {name: tensor} -> path/<name>.npy; float64 stays float64, everything else is written as float32.  When the
+    total exceeds DUMP_BYTES every array is cut to the same fraction of its elements, chosen by a fixed seed."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    arrays = {k: v.detach().to("cpu", torch.float64 if v.dtype == torch.float64 else torch.float32) for k, v in arrays.items()}
+    total = sum(v.numel() * v.element_size() for v in arrays.values())
+    for name, v in arrays.items():
+        if total > DUMP_BYTES:
+            keep = max(1, v.numel() * DUMP_BYTES // total)
+            idx = torch.randperm(v.numel(), generator=torch.Generator().manual_seed(0))[:keep].sort().values
+            v = v.reshape(-1)[idx]
+        np.save(os.path.join(path, name + ".npy"), v.numpy())
 
 
 def workload_cfg(pkg, name):
@@ -89,10 +101,10 @@ def workload_cfg(pkg, name):
 # --------------------------------------------------------------------------------------------------
 # CPU arm: the oracle port on the host cores (bounded sample)
 # --------------------------------------------------------------------------------------------------
-def cpu_sample(pkg, name, steps, warmup, sample_div=4):
+def cpu_sample(pkg, name, steps, warmup, sample_div=4, last=None):
     """Times `oracle.port.generator_forward` for ONE image on a 1/sample_div^2 sub-grid of the workload
     (gen and render resolutions divided by sample_div, same 32 samples per ray, same dims) and scales
-    by the pixel ratio.  Returns (images_per_sec, cores, description)."""
+    by the pixel ratio.  Returns (images_per_sec, cores, description); the last pass's outputs go to `last`."""
     from oracle import port
     cores = host_cores()
     torch.set_num_threads(cores)
@@ -111,7 +123,9 @@ def cpu_sample(pkg, name, steps, warmup, sample_div=4):
     with torch.no_grad():
         for i in range(warmup + steps):
             t0 = time.perf_counter()
-            port.generator_forward(params, z, cond, cfg, u, noise, training=True)
+            out = port.generator_forward(params, z, cond, cfg, u, noise, training=True)
+            if last is not None:
+                last.update(rgbs=out["rgbs"], rgbs_render=out["rgbs_render"])
             if i >= warmup:
                 times.append(time.perf_counter() - t0)
     times.sort()
@@ -149,9 +163,12 @@ def run_reference(args, pkg):
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
         return
-    steps = max(3, min(args.steps, 5))
-    warm = 1
-    ips, cores, desc, t = cpu_sample(pkg, args.workload, steps, warm)
+    steps = max(1, args.steps)
+    warm = args.warmup
+    last = {}
+    ips, cores, desc, t = cpu_sample(pkg, args.workload, steps, warm, last=last)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, last)
     cfg = workload_cfg(pkg, args.workload)
     line = {
         "impl": "reference", "metric": METRIC, "value": ips, "unit": UNIT, "n_gpus": args.gpus, "steps": steps,
@@ -309,9 +326,14 @@ def run_gpu(args, pkg):
         os.environ.setdefault("TORCH_NCCL_ASYNC_ERROR_HANDLING", "0")   # the watchdog must not query events of a capturing stream
         dist.init_process_group("nccl", device_id=dev)
 
+    last = {}
+
     def step_resident():
         with torch.no_grad():
-            return G(z_d, cond_d, **kw)["rgbs"]
+            out = G(z_d, cond_d, **kw)
+        last.clear()
+        last.update(out)
+        return out["rgbs"]
 
     def step_e2e():
         with torch.no_grad():
@@ -344,6 +366,8 @@ def run_gpu(args, pkg):
     sampler = ClockSampler(local) if rank == 0 else None
     ms_total = timed(step_resident, args.steps)
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:      # before anything else runs: the graph's output buffers are reused by later replays
+        dump_outputs(args.dump_outputs, {k: v for k, v in last.items() if torch.is_tensor(v) and v.is_floating_point()})
 
     # Per-kernel device time: the same step launched eagerly with a CUDA-event pair around every launch of the
     # C ABI (a captured graph cannot carry timing events).  Also counts this library's launches per step.
@@ -440,7 +464,7 @@ def run_gpu(args, pkg):
         else:
             roof = {"bound": "tensor", "achieved": fl / sec / 1e12, "peak": pk["bf16_tflops"], "unit": "TFLOP/s"}
         roof["frac"] = roof["achieved"] / roof["peak"]
-        roof.update(kernel=dom, traffic=ncu_traffic(dom, args.workload), peak_source=pk["_source"], algorithmic_flops_per_launch=fl,
+        roof.update(kernel=dom, traffic=None, peak_source=pk["_source"], algorithmic_flops_per_launch=fl,
                     algorithmic_bytes_per_launch=by, mma_passes=int(mult),
                     tensor_frac_issued=fl * mult / sec / (pk["bf16_tflops"] * 1e12),
                     hbm_frac=by / sec / (pk["hbm_gbs"] * 1e9))
@@ -453,12 +477,14 @@ def run_gpu(args, pkg):
     line = {
         "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": max(args.warmup, 3),
         "ms_per_step": ms_total / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-        "dtype": "f32 (bf16x3 split on tcgen05, fp32 accumulate)" if passes_mode == "fp32x3" else "bf16",
+        "dtype": "f32 (bf16x3 split on wgmma, fp32 accumulate)" if passes_mode == "fp32x3" else "bf16",
         "data": "synthetic",
         "config": {"workload": describe(cfg, args.workload, B), "global_batch": B * world,
                    "parallelism": f"dp{world} (SyncBatchNorm statistics all-reduced over NCCL)" if world > 1 else "single GPU",
-                   "l2": "every synthesis activation is %.2f GB (>> 126 MB L2): inputs larger than L2, no flush needed"
-                         % (B * 256 * cfg["gen_height"] * cfg["gen_width"] * 4 / 1e9),
+                   "l2": "every synthesis activation is %.2f GB (>> %d MB L2): inputs larger than L2, no flush needed"
+                         % (B * 256 * cfg["gen_height"] * cfg["gen_width"] * 4 / 1e9,
+                            torch.cuda.get_device_properties(dev).L2_cache_size >> 20),
+                   "gpu": torch.cuda.get_device_name(dev),
                    "precision": passes_mode,
                    "launch": "eager" if (args.no_graph or getattr(G, "_graph_broken", False)) else
                    "whole forward replayed as one CUDA graph" + (" (NCCL all-reduces captured)" if world > 1 else "")},
@@ -518,7 +544,7 @@ def run_gpu(args, pkg):
     _leave(world, G)
 
 
-def train_leg(args, pkg, dev, rank, world, B, steps, warm, precision, split):
+def train_leg(args, pkg, dev, rank, world, B, steps, warm, precision, split, dump=None):
     """BASELINE.json's second metric: one G+D training iteration (discriminator step, then generator step) per step through
     `train_step.Trainer` -- the mirror of the reference's PhaseTrainer (DDP wrappers with their gradient all-reduce over
     NCCL when world > 1, SyncBatchNorm statistics all-reduced inside the generator, five Adam groups, clip, EMA, R1 on its
@@ -550,8 +576,10 @@ def train_leg(args, pkg, dev, rank, world, B, steps, warm, precision, split):
     resident["cond"] = {k: v.to(dev) for k, v in cond_h.items()}
     loss_h = torch.empty(2).pin_memory()
 
+    last = {}
+
     def step_resident():
-        return trainer.iteration(resident)
+        last["d_loss"], last["g_loss"] = trainer.iteration(resident)
 
     def step_e2e():
         batch = {k: v.to(dev, non_blocking=True) for k, v in host.items()}
@@ -591,6 +619,8 @@ def train_leg(args, pkg, dev, rank, world, B, steps, warm, precision, split):
     abi.LAUNCHES = 0
     ms_total = timed(step_resident, steps, record=True)
     launches = abi.LAUNCHES
+    if dump and rank == 0:       # the losses of the last timed iteration
+        dump_outputs(dump, {k: torch.as_tensor(v).to(torch.float64).reshape(1) for k, v in last.items()})
     clocks = sampler.stop() if sampler else None
     ms_e2e = timed(step_e2e, steps)
     finite = bool(torch.isfinite(loss_h).all())
@@ -619,7 +649,7 @@ def train_leg(args, pkg, dev, rank, world, B, steps, warm, precision, split):
     return {
         "metric": "images_per_sec_GD_train_step_512x512", "value": imgs / (ms_total / 1e3), "unit": UNIT, "n_gpus": world,
         "steps": steps, "warmup": warm, "ms_per_step": ms_total / steps, "scaling": "weak",
-        "dtype": "f32 (bf16x3 split on tcgen05, fp32 accumulate)" if precision == "fp32x3" else "bf16 products, fp32 storage",
+        "dtype": "f32 (bf16x3 split on wgmma, fp32 accumulate)" if precision == "fp32x3" else "bf16 products, fp32 storage",
         "config": {"workload": f"C3: one discriminator step + one generator step per iteration (train_step.Trainer = PhaseTrainer's "
                                f"steps: segmentation loss, R1 on its 2-of-8 phase schedule with r1_lambda = {cfg['r1_lambda']} as in "
                                f"configs/map3d.py:98-191, five Adam groups, grad clip 1, EMA), {B} images/GPU/iteration in {split} "
@@ -637,10 +667,10 @@ def train_leg(args, pkg, dev, rank, world, B, steps, warm, precision, split):
                          "r1_iterations_timed": len(ms_r1), "plain_iterations_timed": len(ms_plain),
                          "schedule": "do_r1 on 2 of 8 phases (configs/map3d.py:104-113)",
                          "host_enqueue_ms": sum(host_ms) / max(1, len(host_ms))},
-        "roofline": {"bound": "tensor", "achieved": eq_tflops / world, "peak": pk["bf16_tflops_sustained"], "unit": "TFLOP/s",
-                     "frac": eq_tflops / world / pk["bf16_tflops_sustained"], "traffic": None,
+        "roofline": {"bound": "tensor", "achieved": eq_tflops / world, "peak": pk["bf16_tflops"], "unit": "TFLOP/s",
+                     "frac": eq_tflops / world / pk["bf16_tflops"], "traffic": None, "peak_source": pk["_source"],
                      "note": "reference-equivalent FLOPs of the whole iteration (10.8 TFLOP/image, SURVEY.md 8d) per GPU vs the "
-                             "sustained bf16 tensor peak; fp32x3 issues 3 MMA passes per product"},
+                             "bf16 tensor peak; fp32x3 issues 3 MMA passes per product"},
         "kernels": {k: {"ms_per_step": v[0], "launches_per_step": v[1]} for k, v in sorted(per.items(), key=lambda kv: -kv[1][0])},
     }
 
@@ -656,7 +686,8 @@ def run_train(args, pkg):
         os.environ.setdefault("NCCL_DEBUG", "WARN")
         dist.init_process_group("nccl", device_id=dev)
     abi.require_device()
-    leg = train_leg(args, pkg, dev, rank, world, args.train_batch, args.steps, max(args.warmup, 3), args.precision, args.train_split)
+    leg = train_leg(args, pkg, dev, rank, world, args.train_batch, args.steps, max(args.warmup, 3), args.precision, args.train_split,
+                    dump=args.dump_outputs)
     if rank == 0:
         leg.update(higher_is_better=True, vs_baseline=None, data="synthetic", cpu_baseline=None)
         emit(leg)
@@ -691,8 +722,11 @@ def main():
     ap.add_argument("--no-train", action="store_true", help="skip the G+D training-iteration leg of the default run")
     ap.add_argument("--no-train-bf16", action="store_true", help="skip the additional bf16 training-iteration leg")
     ap.add_argument("--train-batch", type=int, default=16, help="images per GPU per training iteration (config C3: 16)")
-    ap.add_argument("--train-split", type=int, default=2, help="micro-batches per iteration (the reference's batch_split)")
+    ap.add_argument("--train-split", type=int, default=4,
+                    help="micro-batches per iteration (the reference's batch_split; 4 micro-batches of 4 images fit 80 GB)")
     ap.add_argument("--train-steps", type=int, default=4, help="timed training iterations in the default run")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step to DIR/<name>.npy (at most 64 MB in all)")
     args = ap.parse_args()
     claim_stdout()
     pkg = importlib.import_module("3dhumangan_b200")

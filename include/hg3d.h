@@ -1,4 +1,4 @@
-/* hg3d.h -- C ABI of lib3dhg_sm100a.so: the B200-native (sm_100a) kernels behind the 3DHumanGAN
+/* hg3d.h -- C ABI of lib3dhg_sm90a.so: the H100-native (sm_90a) kernels behind the 3DHumanGAN
  * generator / discriminator hot path.
  *
  * Boundary contract (SURVEY.md section 8b; the reference's own native boundary is the pybind11
@@ -29,7 +29,7 @@ extern "C" {
 /* ---- library state -------------------------------------------------------------------------- */
 const char* hg_last_error(void);
 int hg_abi_version(void);
-int hg_check_device(void); /* 0 iff the current device is an sm_100 part */
+int hg_check_device(void); /* 0 iff the current device is an sm_90 part */
 
 /* ---- packed tensor-core weights --------------------------------------------------------------
  * W [N,K] fp32 (row stride ldw) * scale (* *scale_dev when non-null, a DEVICE scalar such as the
@@ -205,7 +205,8 @@ int hg_bilinear_adjoint(const float* da1, float* dp, long dp_stride, int B, int 
  * unet_discriminators.py:21-38), `ntaps` filter taps per launch:
  *   dw[t, r, c] = sum_{b,h,w} dy[b, co0+r, h, w] * x[b, ci0+c, h+oy[t], w+ox[t]]   (zero outside the image)
  * for r < nco <= 256, c < nci <= 256; dw is [ntaps, 256, ceil32(nci)] (unused rows / columns zero), dbias [256] = sum dy
- * (NULL = skip).  ntaps * (nco > 128 ? 2 : 1) * ceil32(nci) <= 512 (TMEM columns); oy / ox are HOST arrays of shifts in
+ * (NULL = skip).  ntaps * (nco > 128 ? 2 : 1) * N <= 256 with N = ceil32(nci) rounded up to 64, 128 or 256 (register
+ * accumulators); oy / ox are HOST arrays of shifts in
  * -1..1; larger filters / channel counts are chunked by the caller (abi.conv2d_wgrad).
  * workspace: hg_conv2d_wgrad_workspace_bytes() bytes of device memory. */
 size_t hg_conv2d_wgrad_workspace_bytes(void);
@@ -220,7 +221,7 @@ int hg_conv2d_wgrad_layer(const float* dy, const float* x, float* dW, float* dbi
                           int H, int W, int Cout, int Cin, int ksize, int passes, void* stream);
 /* 3x3 weight gradient on image rows of >= 128 pixels (W % 128 == 0): the input is converted once per image row into the
  * forward kernel's pixel-major operand image and read as an MN-major B operand, a tap being a row offset of the descriptor.
- * dw [ntaps,128,64] for output channels co0..co0+nco (<= 128) x input channels ci0..ci0+nci (<= 64), ntaps <= 8 taps with
+ * dw [ntaps,128,64] for output channels co0..co0+nco (<= 128) x input channels ci0..ci0+nci (<= 64), ntaps <= 4 taps with
  * shifts (tdy[t], tdx[t]) in {-1,0,1} (host arrays); dbias [128] or NULL.  Same autograd contract as above. */
 size_t hg_conv3x3_wgrad_halo_workspace_bytes(void);
 int hg_conv3x3_wgrad_halo(const float* dy, const float* x, float* dw, float* dbias, void* workspace, int B, int H, int W,

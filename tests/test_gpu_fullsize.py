@@ -1,7 +1,7 @@
 """Parity at the BENCHMARKED sizes (BASELINE.json configs C2 / C3 / C5), not only on the tiny fixtures.
 
 At C2 every persistent CTA of the synthesis kernels walks ~28 tiles per image and the render kernel ~16 per image (ring-phase
-wraps, TMEM half alternation, many tiles per CTA) -- code paths the 32x32 fixtures never reach.  The checker is the
+wraps, accumulator drains, many tiles per CTA) -- code paths the 32x32 fixtures never reach.  The checker is the
 oracle (`oracle/port.py`, pinned to the unmodified reference by tests/test_oracle_pin.py) executed ON THE GPU in plain
 fp32 torch with TF32 disabled; B = 2 keeps it to a few seconds.  Tolerance: 1e-3 relative L2 (the north_star's
 "within 1e-3 relative fp32"); nearest-vertex indices bit-exact.

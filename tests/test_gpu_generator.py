@@ -1,4 +1,4 @@
-"""End to end: Map3DGenerator (module surface -> C ABI -> sm_100a kernels) against the golden vectors
+"""End to end: Map3DGenerator (module surface -> C ABI -> sm_90a kernels) against the golden vectors
 produced by the unmodified reference (tests/golden) and against the oracle."""
 import importlib
 

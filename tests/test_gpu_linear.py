@@ -1,4 +1,4 @@
-"""tcgen05 primitives end to end: weight packing + hg_linear vs a plain fp32 torch reference."""
+"""wgmma primitives end to end: weight packing + hg_linear vs a plain fp32 torch reference."""
 import pytest
 import torch
 

@@ -1,4 +1,4 @@
-"""bias_act / upfirdn2d (sm_100a) against the restated reference implementations."""
+"""bias_act / upfirdn2d (sm_90a) against the restated reference implementations."""
 import importlib
 
 import pytest

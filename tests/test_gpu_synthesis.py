@@ -1,4 +1,4 @@
-"""SPADE synthesis network on the tcgen05 kernels vs the oracle (train-mode BatchNorm, fp32 contract 1e-3)."""
+"""SPADE synthesis network on the wgmma kernels vs the oracle (train-mode BatchNorm, fp32 contract 1e-3)."""
 from importlib import import_module
 
 import pytest

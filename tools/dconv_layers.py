@@ -1,5 +1,5 @@
 """Per-layer device time of the discriminator's convolutions (inference path, B images at size x size): shape, kernel
-variant, ms, reference-equivalent TFLOP/s and issued fraction of the bf16 tensor peak.  Needs a B200.
+variant, ms, reference-equivalent TFLOP/s and issued fraction of the bf16 tensor peak.  Needs an H100.
     python tools/dconv_layers.py [--batch 8] [--size 512] [--precision fp32x3]"""
 import argparse
 import importlib

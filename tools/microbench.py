@@ -4,7 +4,7 @@ discriminator forward (a14, tensor-pipe bound), bias_act / upfirdn2d (a'1, a'2, 
     python tools/microbench.py [--batch 8] [--iters 10] > gpurun_out/micro.json
 
 Prints one JSON object; every number is CUDA-event time on the launching stream after warm-up, inputs
-larger than L2 (or an L2 flush between iterations for the small ops).  Needs a B200 and the built library.
+larger than L2 (or an L2 flush between iterations for the small ops).  Needs an H100 and the built library.
 """
 import argparse
 import importlib
