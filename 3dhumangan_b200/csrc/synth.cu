@@ -75,7 +75,7 @@ struct SpadeArgs {
   int cout;              // output channels written by the epilogue: 256 or 128 (the MMA always runs N = 256)
   int out_pm;            // backward epilogue: write pixel-major [B,HW,cout] instead of tile-blocked
   int act;               // 0: LeakyReLU(slope) (SPADE), 1: sine (FiLM-SIREN layers of the renderer: y = sin(x*g1 + g0))
-  const float* ascale;   // backward operand: per-(b,c) scale [B,C] applied to the incoming gradient, or null
+  const float* ascale;   // backward operand: per-(b,c) scale [B,C] applied to the incoming gradient ([B,2C] with x2), or null
   const float* rk_v;     // backward epilogue: rank-k term  acc += sum_j rgb_w[j][c] * rk_v[b][j][pixel]  (k = rk_n <= 3)
   int rk_n;
   const float* mod2;     // forward, K = 512: [B,2,C] table of the SECOND source's channels (null: the first table serves both,
@@ -558,7 +558,11 @@ __global__ void __launch_bounds__(kSynThreads, 1) spade_const_kernel(SpadeArgs a
         if (kBwd && cur_b >= 0) flush_bwd_sums(a, m, cur_b);
         for (int i = threadIdx.x; i < kC; i += 256) {
           if (kBwd) {
-            if (a.ascale) m.tab_as[i] = a.ascale[static_cast<long>(b) * kC + i];
+            if (a.ascale) {    // K = 512: columns kC.. scale g2; they live in the (pixel-style only) gamma/beta bias table
+              const long ld = a.x2 ? 2 * kC : kC;
+              m.tab_as[i] = a.ascale[static_cast<long>(b) * ld + i];
+              if (a.x2) m.tab_bgb[i] = a.ascale[static_cast<long>(b) * ld + kC + i];
+            }
             if (i < a.cout) {
               m.tab_g1[i] = a.mod ? a.mod[(static_cast<long>(b) * 2 + 0) * a.cout + i] : 1.f;
               m.tab_g0[i] = a.mod ? a.mod[(static_cast<long>(b) * 2 + 1) * a.cout + i] : 0.f;
@@ -584,7 +588,7 @@ __global__ void __launch_bounds__(kSynThreads, 1) spade_const_kernel(SpadeArgs a
       opaque(tg0b);
       const float slope = a.slope;
       const bool sine = a.act == 1, scaled = kBwd && a.ascale != nullptr;
-      const bool two_tables = !kBwd && a.mod2 != nullptr;
+      const bool two_tables = kBwd ? (scaled && a.x2 != nullptr) : a.mod2 != nullptr;
 #pragma unroll 1
       for (int kc = 0; kc < a.nkc; ++kc, ++acnt) {
         const int c0 = (kc * 64 + h * 32) & (kC - 1);
@@ -1057,7 +1061,6 @@ int hg_conv1x1_blocked_bwd(const float* g, const float* g2, const float* aux, co
                            const float* rk_w, const float* rk_v, int rk_n, int B, int Hg, int Wg, int passes,
                            void* stream) {
   HG_REQUIRE(act == 0 || act == 1, "hg_conv1x1_blocked_bwd: act must be 0 (LeakyReLU/ReLU mask) or 1 (cosine)");
-  HG_REQUIRE(!ascale || !g2, "hg_conv1x1_blocked_bwd: the operand scale is built for K = 256");
   HG_REQUIRE(!rk_v || (rk_w && rk_n >= 1 && rk_n <= 3 && Cout == 256), "hg_conv1x1_blocked_bwd: bad rank-k term");
   HG_REQUIRE(g && aux && wimg_t && out && sums, "hg_conv1x1_blocked_bwd: null pointer");
   HG_REQUIRE(Cout == 128 || Cout == 256, "hg_conv1x1_blocked_bwd: Cout must be 128 or 256 (got %d)", Cout);

@@ -335,12 +335,9 @@ class Map3DGenerator(nn.Module):
         cond = {k: conditions[k] for k in ("skeletons_xyz", "vertices", "tpose_vertices", "fk_matrices", "lbs_weights",
                                            "cam2world_matrices", "intrinsics", "scales")}
         u, noise = rng.draw_render_noise(B, Rh * Rw, S, dev, cfg.get("sample_dist", None))
-        if self.hidden_dim != 256:
+        if self.hidden_dim != 256 and not self._wants_grad():
             # hidden_dim 384 (MAP3DBN) / 420 (MAP3DBN512L, the released checkpoint): the zero-padded 2 x 256 path on the
-            # general blocked-GEMM engine (modules/wide_ops.py); forward only
-            if self._wants_grad():
-                raise RuntimeError("hg3d: gradients are built for hidden_dim == 256 (the 512-pixel curricula); hidden_dim "
-                                   f"{self.hidden_dim} runs forward only -- call it under torch.no_grad()")
+            # general blocked-GEMM engine (modules/wide_ops.py); under autograd it runs inside GeneratorCore below
             from . import wide_ops
             feats, rgb01, depth = wide_ops.render_forward_wide(P, freq, phase, cond, cfg, u, noise, passes=passes)
             rgb = wide_ops.synthesis_forward_wide(P, feats, styles.reshape(B, -1), cfg, training=self.training, passes=passes)

@@ -252,14 +252,21 @@ class GeneratorCore(torch.autograd.Function):
             raise RuntimeError("hg3d: the training renderer is built for hierarchical_sample=False, lock_view_dependence=True")
         if cfg.get("neural_field_blocks", 4) != 4:
             raise RuntimeError("hg3d: the training renderer is built for neural_field_blocks == 4 (all shipped curricula)")
-        rec, z_vals = geo_records(cond, cfg, u)
-        with torch.enable_grad():
-            ray, rtape = mlp_forward_train(P, freq, phase, rec, z_vals, noise, cfg, geo_dim=cfg["geo_feature_dim"],
-                                           passes=passes)
-            rgb, stape = synthesis_train.synthesis_forward_train(P, ray, styles.reshape(B, -1), cfg, passes=passes)
+        if cfg["hidden_dim"] != H:      # 384 / 420: the zero-padded forward of wide_ops with tapes, backward in wide_train
+            from . import wide_ops
+            rtape, stape = {}, synthesis_train.SynthesisTape()
+            feats, rgb01, depth = wide_ops.render_forward_wide(P, freq, phase, cond, cfg, u, noise, passes=passes, tape=rtape)
+            rgb = wide_ops.synthesis_forward_wide(P, feats, styles.reshape(B, -1), cfg, training=True, passes=passes, tape=stape)
+            rgb_render = (rgb01 * 2 - 1).reshape(B, Rh, Rw, 3).permute(0, 3, 1, 2).contiguous()
+        else:
+            rec, z_vals = geo_records(cond, cfg, u)
+            with torch.enable_grad():
+                ray, rtape = mlp_forward_train(P, freq, phase, rec, z_vals, noise, cfg, geo_dim=cfg["geo_feature_dim"],
+                                               passes=passes)
+                rgb, stape = synthesis_train.synthesis_forward_train(P, ray, styles.reshape(B, -1), cfg, passes=passes)
+            rgb_render = (ray[..., 256:259] * 2 - 1).reshape(B, Rh, Rw, 3).permute(0, 3, 1, 2).contiguous()
+            depth = ray[..., 259:260].contiguous()
         ctx.tapes = (P, rtape, stape, cfg, passes, names)
-        rgb_render = (ray[..., 256:259] * 2 - 1).reshape(B, Rh, Rw, 3).permute(0, 3, 1, 2).contiguous()
-        depth = ray[..., 259:260].contiguous()
         ctx.mark_non_differentiable(depth)
         return rgb, rgb_render, depth
 
@@ -275,15 +282,22 @@ class GeneratorCore(torch.autograd.Function):
         B = stape.B
         Rh, Rw = cfg["render_height"], cfg["render_width"]
         grads = {}
-        with torch.enable_grad():
-            dfs, dfeat = synthesis_train.synthesis_backward(P, stape, d_rgb, passes=passes, grads=grads)
-        dray = torch.zeros(B, Rh * Rw, 260, dtype=torch.float32, device=d_rgb.device)
-        if dfeat is not None:
-            dray[..., :256] = dfeat
-        if d_rgb_render is not None:
-            dray[..., 256:259] = 2.0 * d_rgb_render.permute(0, 2, 3, 1).reshape(B, Rh * Rw, 3)
-        with torch.enable_grad():
-            dfreq, dphase = mlp_backward(rtape, dray, grads=grads)
+        if cfg["hidden_dim"] != H:
+            from . import wide_train
+            with torch.enable_grad():
+                dfs, dfeat = wide_train.synthesis_backward_wide(P, stape, d_rgb, passes=passes, grads=grads)
+                drgb = None if d_rgb_render is None else 2.0 * d_rgb_render.permute(0, 2, 3, 1).reshape(B, Rh * Rw, 3)
+                dfreq, dphase = wide_train.render_backward_wide(rtape, dfeat, drgb, grads=grads)
+        else:
+            with torch.enable_grad():
+                dfs, dfeat = synthesis_train.synthesis_backward(P, stape, d_rgb, passes=passes, grads=grads)
+            dray = torch.zeros(B, Rh * Rw, 260, dtype=torch.float32, device=d_rgb.device)
+            if dfeat is not None:
+                dray[..., :256] = dfeat
+            if d_rgb_render is not None:
+                dray[..., 256:259] = 2.0 * d_rgb_render.permute(0, 2, 3, 1).reshape(B, Rh * Rw, 3)
+            with torch.enable_grad():
+                dfreq, dphase = mlp_backward(rtape, dray, grads=grads)
         ctx.tapes = None
         # Every returned gradient must own its storage: autograd's AccumulateGrad steals a returned tensor as `.grad` when
         # nobody else holds the TensorImpl, so two parameters whose gradients are views of one buffer (the nine ToRGB biases

@@ -100,11 +100,7 @@ def synthesis_forward_train(params, feat_lr, fixed_style, cfg, *, passes=3, pref
     for k, j in halves:
         if (k, j) in pxi:
             continue
-        s = sp(k, j)
-        actv = torch.relu(F.linear(fs, P[s + "mlp_shared.0.weight"].reshape(128, C), P[s + "mlp_shared.0.bias"]))
-        G = 1.0 + F.linear(actv, P[s + "mlp_gamma.weight"].reshape(C, 128), P[s + "mlp_gamma.bias"])
-        Bt = F.linear(actv, P[s + "mlp_beta.weight"].reshape(C, 128), P[s + "mlp_beta.bias"])
-        GB[(k, j)] = (G, Bt)
+        GB[(k, j)] = const_gamma_beta(P, sp(k, j), fs, C)
 
     # ---- synthesis input (shared by the batch) + its statistics
     stats = torch.zeros(len(halves) + 1, STAT_STRIDE, dtype=torch.float64, device=dev)
@@ -131,22 +127,8 @@ def synthesis_forward_train(params, feat_lr, fixed_style, cfg, *, passes=3, pref
         # leaves of the batch statistics: their gradients are the a[c], k[c] of dL/dx
         ssum = srow[:C].clone().requires_grad_(True)
         ssq = srow[C:2 * C].clone().requires_grad_(True)
-        mean = ssum / count
-        var = (ssq / count - mean * mean).clamp_min(0.0)
-        rstd = torch.rsqrt(var + 1e-5)
-        sc = P[bn + "weight"].double() * rstd
-        sh = P[bn + "bias"].double() - mean * sc
         pixel = (k, j) in pxi
-        if pixel:       # BatchNorm scale/shift only; gamma/beta are per pixel
-            mod = torch.stack([sc, sh]).float()                                                                 # [2,C]
-        else:
-            G, Bt = GB[(k, j)]
-            mod = torch.stack([sc[None, :] * G.double(), sh[None, :] * G.double() + Bt.double()], dim=1).float()   # [B,2,C]
-        with torch.no_grad():       # running statistics (momentum 0.1, unbiased variance), map3d_layers.py:162
-            P[bn + "running_mean"].mul_(0.9).add_(0.1 * mean.float())
-            P[bn + "running_var"].mul_(0.9).add_(0.1 * (var * count / max(count - 1, 1)).float())
-            if (bn + "num_batches_tracked") in P:
-                P[bn + "num_batches_tracked"] += 1
+        mod = spade_table(P, bn, ssum, ssq, count, None if pixel else GB[(k, j)])
         conv = blk(k) + f"conv_{j}."
         w_sn = w_sns[conv].reshape(C, C)
         wimg = abi.pack_weight(w_sn.detach().contiguous(), Nb=256)[0]
@@ -187,6 +169,38 @@ def synthesis_forward_train(params, feat_lr, fixed_style, cfg, *, passes=3, pref
         cur, cur_bstride = out, T * C * 128
     tape.rgb = rgb_cur.reshape(B, 3, Hg, Wg)
     return tape.rgb, tape
+
+
+def const_gamma_beta(P, s, fs, C):
+    """(1 + gamma, beta) [B,C] of a const-style SPADE from the fixed style fs [B,C], with autograd history
+    (SPADE2d.forward, map3d_layers.py:176-190)."""
+    actv = torch.relu(F.linear(fs, P[s + "mlp_shared.0.weight"].reshape(128, C), P[s + "mlp_shared.0.bias"]))
+    G = 1.0 + F.linear(actv, P[s + "mlp_gamma.weight"].reshape(C, 128), P[s + "mlp_gamma.bias"])
+    Bt = F.linear(actv, P[s + "mlp_beta.weight"].reshape(C, 128), P[s + "mlp_beta.bias"])
+    return G, Bt
+
+
+def spade_table(P, bn, ssum, ssq, count, gb=None):
+    """The folded BatchNorm (+ SPADE) table of one half-block with autograd history from the batch-statistics leaves
+    ssum = sum(x), ssq = sum(x^2) [C]: [2,C] = (sc, sh) for pixel style (gb None), else [B,2,C] = (sc*G, sh*G + beta) with
+    gb = (G, beta) from `const_gamma_beta`.  Updates the running statistics (momentum 0.1, unbiased variance,
+    map3d_layers.py:162)."""
+    mean = ssum / count
+    var = (ssq / count - mean * mean).clamp_min(0.0)
+    rstd = torch.rsqrt(var + 1e-5)
+    sc = P[bn + "weight"].double() * rstd
+    sh = P[bn + "bias"].double() - mean * sc
+    if gb is None:      # BatchNorm scale/shift only; gamma/beta are per pixel
+        mod = torch.stack([sc, sh]).float()
+    else:
+        G, Bt = gb
+        mod = torch.stack([sc[None, :] * G.double(), sh[None, :] * G.double() + Bt.double()], dim=1).float()
+    with torch.no_grad():
+        P[bn + "running_mean"].mul_(0.9).add_(0.1 * mean.float())
+        P[bn + "running_var"].mul_(0.9).add_(0.1 * (var * count / max(count - 1, 1)).float())
+        if (bn + "num_batches_tracked") in P:
+            P[bn + "num_batches_tracked"] += 1
+    return mod
 
 
 def grad_accumulator(P, grads):

@@ -15,18 +15,20 @@ affine and zero FiLM tables, so they stay zero through every layer.
              gamma / beta by `hg_conv1x1_blocked`, pre = BN(x) * gamma + beta (`hg_spade_pixel_pre`), then the wide conv with
              an identity table -- the decomposition the 256-channel BACKWARD already uses.
 
-Inference and train-mode forward (batch statistics, running-stat and spectral-norm buffer updates); gradients for these
-widths are not built (the module raises).  Mirrors Map3DGenerator.render / forward (map3d_generator.py:208-280, 381-523),
+Inference and train-mode forward (batch statistics, running-stat and spectral-norm buffer updates).  Given a `tape`,
+each forward also keeps what its backward (modules/wide_train.py) needs, and builds the small tables that carry
+parameter gradients (FiLM, SPADE / BatchNorm, W / sigma) with autograd history.  Mirrors Map3DGenerator.render / forward (map3d_generator.py:208-280, 381-523),
 COORDCONCATSIREN.forward (modulated.py:41-75), SynthesisNetwork.forward (map3d_generator.py:58-97).
 """
 from __future__ import annotations
 
 import torch
 import torch.distributed as dist
+import torch.nn.functional as F
 
 from .. import abi
 from ..ops.dense import _gemm_nt
-from .synthesis_ops import STAT_STRIDE, _PtrView, all_reduce_stats, is_pixel_style, spectral_sigma_batched
+from .synthesis_ops import STAT_STRIDE, _PtrView, all_reduce_stats, is_pixel_style, sn_weights, spectral_sigma_batched
 
 HALF = 256
 
@@ -79,8 +81,10 @@ def wide_layer(xs, W512, b512, *, mods=None, act=0, slope=0.2, skips=None, stats
 # renderer
 # ----------------------------------------------------------------------------------------------------------------------
 @torch.no_grad()
-def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix="neural_field."):
-    """-> ray features [B,R,C], rgb [B,R,3] (in [0,1], before the *2-1), depth [B,R,1]."""
+def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix="neural_field.", tape=None):
+    """-> ray features [B,R,C], rgb [B,R,3] (in [0,1], before the *2-1), depth [B,R,1].
+    `tape` (a dict) receives what `wide_train.render_backward_wide` needs: per half the linear outputs lin_a, lin_b,
+    out_0..3, lin_c, feat, then sig, rgbp and the FiLM tables built from freq / phase leaves with autograd history."""
     from . import render_train
     abi.require_device()
     g = lambda n: P[prefix + n].detach().float()
@@ -90,6 +94,8 @@ def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix
         raise RuntimeError("hg3d: the zero-padded path serves hidden_dim <= 512")
     if cfg.get("neural_field_blocks", 4) != 4:
         raise RuntimeError("hg3d: the renderer is built for neural_field_blocks == 4 (all shipped curricula)")
+    if tape is not None and cfg.get("last_back", False):
+        raise RuntimeError("hg3d: last_back=True is an inference-only setting (eval_last_back); the training renderer does not build it")
     dev = freq.device
     B = freq.shape[0]
     S = cfg["num_steps"]
@@ -106,16 +112,20 @@ def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix
     rec_b = render_train.blocked_points(rec[..., :3 + geo_dim], 128)
 
     # FiLM tables per half [B,2,256]: (f, phi), zero in the padded channels so that sin(0 * x + 0) = 0
-    f = freq.float() * 15 + 30
-    ph = phase.float()
+    taped = tape is not None
+    with torch.set_grad_enabled(taped):
+        fq = freq.detach().float().requires_grad_(taped)
+        ph = phase.detach().float().requires_grad_(taped)
+        f = fq * 15 + 30
 
-    def table(fv, pv):
-        t = torch.zeros(B, 2, 2 * HALF, **f32)
-        t[:, 0, :C] = fv
-        t[:, 1, :C] = pv
-        return t[:, :, :HALF].contiguous(), t[:, :, HALF:].contiguous()
+        def table(fv, pv):
+            t = torch.zeros(B, 2, 2 * HALF, **f32)
+            t[:, 0, :C] = fv
+            t[:, 1, :C] = pv
+            return t[:, :, :HALF].contiguous(), t[:, :, HALF:].contiguous()
 
-    mods = [table(f[:, i * C:(i + 1) * C], ph[:, i * C:(i + 1) * C]) for i in range(4)]
+        mods_h = [table(f[:, i * C:(i + 1) * C], ph[:, i * C:(i + 1) * C]) for i in range(4)]
+    mods = [(lo.detach(), hi.detach()) for lo, hi in mods_h]
     m30 = table(torch.full((B, C), 30.0, **f32), torch.zeros(B, C, **f32))
 
     # first layers: K = 3 / 31 zero-padded to 128 input channels
@@ -131,8 +141,13 @@ def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix
     zero_b = torch.zeros(2 * HALF, **f32)
     part = wide_layer(lin_a, _pad2(w0[:, :C], 2 * HALF, 2 * HALF), _pad1(g("network.0.layer.bias"), 2 * HALF), mods=m30, act=1, **kw)
     x = wide_layer(lin_b, _pad2(w0[:, C:], 2 * HALF, 2 * HALF), zero_b, mods=m30, act=1, skips=part, **kw)
+    if taped:
+        tape.update(rec_b=rec_b, lin_a=lin_a, lin_b=lin_b, m30=m30)
     del part, lin_a, lin_b
+    outs = []
     for i in range(1, 4):
+        if taped:
+            outs.append(x)
         x = wide_layer(x, _pad2(g(f"network.{i}.layer.weight"), 2 * HALF, 2 * HALF), _pad1(g(f"network.{i}.layer.bias"), 2 * HALF),
                        mods=mods[i - 1], act=1, **kw)
     out3 = x
@@ -158,6 +173,13 @@ def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix
                 softplus=cfg["clamp_mode"] == "softplus", last_back=cfg.get("last_back", False))
     ray0, _ = abi.render_composite(sig, z_vals, nz, rgbp, feat[0], **comp)
     ray1, _ = abi.render_composite(sig, z_vals, nz, rgbp, feat[1], **comp)
+    if taped:
+        with torch.enable_grad():      # colour bias and direction columns, with history (cf. render_train.mlp_forward_train)
+            bcol_t = P[prefix + "color_layer_sine.layer.bias"] + P[prefix + "color_layer_sine.layer.weight"][:, :3] @ dvec
+        del comp["last_back"]
+        tape.update(P=P, prefix=prefix, C=C, Fd=Fd, B=B, N=N, R=R, geo_dim=geo_dim, kw=kw, fq=fq, ph=ph, mods_h=mods_h, mods=mods,
+                    outs=outs + [out3], lin_c=lin_c, feat=feat, sig=sig, rgbp=rgbp, z=z_vals, noise=nz, comp=comp, bcol=bcol_t,
+                    w_sigma=w_sigma, w_rgb=w_rgb)
     feats = torch.cat([ray0[..., :HALF], ray1[..., :HALF]], -1)[..., :Fd].contiguous()
     return feats, ray0[..., 256:259].contiguous(), ray0[..., 259:260].contiguous()
 
@@ -167,8 +189,11 @@ def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix
 # ----------------------------------------------------------------------------------------------------------------------
 @torch.no_grad()
 def synthesis_forward_wide(P, feats, fixed_style, cfg, *, training=True, passes=3, prefix="synthesis_network.",
-                           input_prefix="synthesis_input.", process_group=None):
-    """feats [B, Rh*Rw, C] render-resolution features, fixed_style [B,C] -> rgb [B,3,Hg,Wg]."""
+                           input_prefix="synthesis_input.", process_group=None, tape=None):
+    """feats [B, Rh*Rw, C] render-resolution features, fixed_style [B,C] -> rgb [B,3,Hg,Wg].
+    `tape` (a `synthesis_train.SynthesisTape`, training only) receives what `wide_train.synthesis_backward_wide` needs: per
+    half-block its input halves, the SPADE tables built with autograd from sum(x) / sum(x^2) leaves (instead of
+    hg_bn_finalize), W / sigma with history and the skip / ToRGB bookkeeping, as `synthesis_train` keeps them."""
     abi.require_device()
     dev = feats.device
     B = feats.shape[0]
@@ -189,18 +214,34 @@ def synthesis_forward_wide(P, feats, fixed_style, cfg, *, training=True, passes=
     kw = dict(B=B, Hg=Hg, Wg=Wg, passes=passes)
 
     conv_names = [blk(k) + f"conv_{j}." for k, j in halves]
-    inv_sigma = spectral_sigma_batched([P[n + "weight_orig"] for n in conv_names], [P[n + "weight_u"] for n in conv_names],
-                                       [P[n + "weight_v"] for n in conv_names], training)
     fs = fixed_style.reshape(B, C).float()
     px = [(k, j) for k, j in halves if is_pixel_style(cfg, k)]
     pxi = {key: i for i, key in enumerate(px)}
+    taped = tape is not None
+    if taped:
+        if not training:
+            raise RuntimeError("hg3d: gradients through the generator are built for train() mode (batch statistics)")
+        with torch.enable_grad():
+            w_sns = sn_weights(P, conv_names, True)
+        fs = fs.detach().requires_grad_(True)           # leaf: its gradient is returned by the backward
+        tape.cfg, tape.B, tape.fixed_style, tape.px = cfg, B, fs, px
+        tape.process_group, tape.world = process_group, world
+    else:
+        inv_sigma = spectral_sigma_batched([P[n + "weight_orig"] for n in conv_names], [P[n + "weight_u"] for n in conv_names],
+                                           [P[n + "weight_v"] for n in conv_names], training)
     p_lr = None
     if px:
         Ws = torch.cat([P[sp(k, j) + "mlp_shared.0.weight"].reshape(128, C) for k, j in px]).float()      # [n*128, C]
         bsh = torch.stack([P[sp(k, j) + "mlp_shared.0.bias"] for k, j in px]).float()
         X = feats.reshape(B * Rh * Rw, feats.shape[-1])[:, :C]
         p_lr = _gemm_nt(X, Ws, passes=passes)                                                              # [B*Rhw, n*128]
-        if mode in ("mixed", "all"):
+        if taped:       # the per-sample constant after the up-sample, with history (cf. synthesis_train)
+            with torch.enable_grad():
+                PB = [F.linear(fs, P[sp(k, j) + "mlp_shared.0.weight"].reshape(128, C), P[sp(k, j) + "mlp_shared.0.bias"])
+                      if mode in ("mixed", "all") else P[sp(k, j) + "mlp_shared.0.bias"][None, :].expand(B, 128) for k, j in px]
+            p_bias = torch.stack([t.detach().float() for t in PB])
+            tape.p = dict(Ws=Ws, X=X, p_lr=p_lr)
+        elif mode in ("mixed", "all"):
             p_bias = (_gemm_nt(fs, Ws, passes=passes)).reshape(B, len(px), 128).permute(1, 0, 2) + bsh[:, None, :]
         else:
             p_bias = bsh[:, None, :].expand(len(px), B, 128)
@@ -220,6 +261,8 @@ def synthesis_forward_wide(P, feats, fixed_style, cfg, *, training=True, passes=
                         stats[0, h] if training else None, B)
         cur.append(x0[None].expand(B, T, HALF, 128).contiguous())
     cur = tuple(cur)
+    if taped:
+        tape.input = dict(w=w_in, b=b_in, ic=ic, jc=jc, prefix=input_prefix)
 
     rgb_cur = None
     block_in = None
@@ -230,49 +273,31 @@ def synthesis_forward_wide(P, feats, fixed_style, cfg, *, training=True, passes=
         if training and world > 1:
             for h in (0, 1):
                 all_reduce_stats(stats[idx, h], process_group)
-        # BatchNorm (+ per-sample SPADE vectors for const style) per half; padded channels get weight = bias = 0
-        bw, bbias = _pad1(P[bn + "weight"].float(), W2), _pad1(P[bn + "bias"].float(), W2)
-        rm, rv = _pad1(P[bn + "running_mean"].float(), W2), _pad1(P[bn + "running_var"].float(), W2, fill=1.0)
-        if not pixel:
-            s = sp(k, j)
-            actv = torch.relu(_gemm_nt(fs, P[s + "mlp_shared.0.weight"].reshape(128, C).float(), passes=passes)
-                              + P[s + "mlp_shared.0.bias"].float())
-            G = 1.0 + _gemm_nt(actv, P[s + "mlp_gamma.weight"].reshape(C, 128).float(), passes=passes) + P[s + "mlp_gamma.bias"].float()
-            Bt = _gemm_nt(actv, P[s + "mlp_beta.weight"].reshape(C, 128).float(), passes=passes) + P[s + "mlp_beta.bias"].float()
-            GB = torch.zeros(B, 2, W2, **f32)
-            GB[:, 0, :C] = G
-            GB[:, 1, :C] = Bt
-        tables = []
-        for h in (0, 1):
-            sl = slice(h * HALF, (h + 1) * HALF)
-            rm_h, rv_h = rm[sl].contiguous(), rv[sl].contiguous()
-            scsh = torch.empty(2, HALF, **f32) if pixel else None
-            mod = None if pixel else torch.empty(B, 2, HALF, **f32)
-            abi.bn_finalize(stats[idx, h] if training else None, bw[sl].contiguous(), bbias[sl].contiguous(), rm_h, rv_h, training,
-                            count_dev=stats[idx, h, 512:513] if training else None, gb=None if pixel else GB[:, :, sl].contiguous(), B=B,
-                            scsh=scsh, mod=mod)
-            if training:
-                rm[sl], rv[sl] = rm_h, rv_h
-            tables.append(scsh if pixel else mod)
-        if training:
-            P[bn + "running_mean"].copy_(rm[:C])
-            P[bn + "running_var"].copy_(rv[:C])
-            if (bn + "num_batches_tracked") in P:
-                P[bn + "num_batches_tracked"] += 1
+        if taped:
+            mod, tables, ssum, ssq = _taped_tables(P, stats[idx], bn, sp(k, j), fs, pixel, C, float(B * HW * world))
+        else:
+            tables = _tables(P, stats[idx], bn, sp(k, j), fs, pixel, C, B, training, passes)
         if j == 0:
             block_in = (cur, idx)
         last_half = j == 1
         use_skip = last_half and k >= nb // 2 and block_in[1] != 0
         use_rgb = last_half and k >= nb // 2 - 1
         conv = blk(k) + f"conv_{j}."
-        Wc = _pad2(P[conv + "weight_orig"].reshape(C, C).float() * inv_sigma[idx], W2, W2)
+        if taped:
+            Wc = _pad2(w_sns[conv].detach().reshape(C, C), W2, W2)
+        else:
+            Wc = _pad2(P[conv + "weight_orig"].reshape(C, C).float() * inv_sigma[idx], W2, W2)
         bc = _pad1(P[conv + "bias"].float(), W2)
-        rgb = None
+        rgb = name = None
         if use_rgb:
             name = f"{prefix}to_rgbs.m3d_{k}.linear."
             rgb = dict(w=_pad2(P[name + "weight"].reshape(3, C).float(), 3, W2), b=P[name + "bias"].float().contiguous(), rgb_in=rgb_cur,
                        out0=torch.empty(B, 3, HW, **f32), out1=torch.empty(B, 3, HW, **f32))
         srows = (stats[idx + 1, 0], stats[idx + 1, 1]) if training else None
+        if taped:
+            rec = dict(x=cur, mod=mod, mod_d=tables, w_sn=w_sns[conv], ssum=ssum, ssq=ssq, conv=conv, pixel=pixel,
+                       skip_from=block_in[1] if use_skip else None, rgb=name, rgb_w=None if rgb is None else rgb["w"])
+            tape.halves.append(rec)
         if pixel:
             i = pxi[(k, j)]
             s_ = sp(k, j)
@@ -282,6 +307,8 @@ def synthesis_forward_wide(P, feats, fixed_style, cfg, *, training=True, passes=
             wb = _pad2(P[s_ + "mlp_beta.weight"].reshape(C, 128).float(), W2, 128)
             bg1 = _pad1(P[s_ + "mlp_gamma.bias"].float() + 1.0, W2)
             bb = _pad1(P[s_ + "mlp_beta.bias"].float(), W2)
+            if taped:
+                rec.update(i=i, spade=s_, p_bias=PB[i], p_bias_d=p_bias[i].contiguous(), wg=wg, wb=wb, bg1=bg1, bb=bb)
             pres = []
             for h in (0, 1):
                 sl = slice(h * HALF, (h + 1) * HALF)
@@ -296,7 +323,60 @@ def synthesis_forward_wide(P, feats, fixed_style, cfg, *, training=True, passes=
         else:
             out = wide_layer(cur, Wc, bc, mods=tuple(tables), act=0, slope=0.2, skips=block_in[0] if use_skip else None, stats=srows,
                              rgb=rgb, **kw)
+        if taped:
+            rec["out"] = out
         if use_rgb:
             rgb_cur = rgb["out1"]
         cur = out
-    return rgb_cur.reshape(B, 3, Hg, Wg)
+    rgb_cur = rgb_cur.reshape(B, 3, Hg, Wg)
+    if taped:
+        tape.rgb = rgb_cur
+    return rgb_cur
+
+
+def _taped_tables(P, srow, bn, s, fs, pixel, C, count):
+    """Training forward with a tape: the SPADE table of one half-block by `synthesis_train.spade_table` from the leaves
+    sum(x), sum(x^2) [512] of its batch statistics (both halves), zero-padded to 512 channels.
+    -> (table [(B,)2,512] with history, its two detached halves, ssum, ssq)."""
+    from .synthesis_train import const_gamma_beta, spade_table
+    ssum = srow[:, :HALF].reshape(2 * HALF).clone().requires_grad_(True)
+    ssq = srow[:, HALF:2 * HALF].reshape(2 * HALF).clone().requires_grad_(True)
+    with torch.enable_grad():
+        mod = spade_table(P, bn, ssum[:C], ssq[:C], count, None if pixel else const_gamma_beta(P, s, fs, C))
+        mod = F.pad(mod, (0, 2 * HALF - C))          # padded channels: g1 = g0 = 0
+    return mod, [mod[..., :HALF].detach().contiguous(), mod[..., HALF:].detach().contiguous()], ssum, ssq
+
+
+def _tables(P, srow, bn, s, fs, pixel, C, B, training, passes):
+    """BatchNorm (+ per-sample SPADE vectors for const style) per half by hg_bn_finalize; padded channels get
+    weight = bias = 0.  -> [table_lo, table_hi]: scsh [2,256] (pixel style) or [B,2,256]."""
+    f32 = dict(dtype=torch.float32, device=fs.device)
+    W2 = 2 * HALF
+    bw, bbias = _pad1(P[bn + "weight"].float(), W2), _pad1(P[bn + "bias"].float(), W2)
+    rm, rv = _pad1(P[bn + "running_mean"].float(), W2), _pad1(P[bn + "running_var"].float(), W2, fill=1.0)
+    if not pixel:
+        actv = torch.relu(_gemm_nt(fs, P[s + "mlp_shared.0.weight"].reshape(128, C).float(), passes=passes)
+                          + P[s + "mlp_shared.0.bias"].float())
+        G = 1.0 + _gemm_nt(actv, P[s + "mlp_gamma.weight"].reshape(C, 128).float(), passes=passes) + P[s + "mlp_gamma.bias"].float()
+        Bt = _gemm_nt(actv, P[s + "mlp_beta.weight"].reshape(C, 128).float(), passes=passes) + P[s + "mlp_beta.bias"].float()
+        GB = torch.zeros(B, 2, W2, **f32)
+        GB[:, 0, :C] = G
+        GB[:, 1, :C] = Bt
+    tables = []
+    for h in (0, 1):
+        sl = slice(h * HALF, (h + 1) * HALF)
+        rm_h, rv_h = rm[sl].contiguous(), rv[sl].contiguous()
+        scsh = torch.empty(2, HALF, **f32) if pixel else None
+        mod = None if pixel else torch.empty(B, 2, HALF, **f32)
+        abi.bn_finalize(srow[h] if training else None, bw[sl].contiguous(), bbias[sl].contiguous(), rm_h, rv_h, training,
+                        count_dev=srow[h, 512:513] if training else None, gb=None if pixel else GB[:, :, sl].contiguous(), B=B,
+                        scsh=scsh, mod=mod)
+        if training:
+            rm[sl], rv[sl] = rm_h, rv_h
+        tables.append(scsh if pixel else mod)
+    if training:
+        P[bn + "running_mean"].copy_(rm[:C])
+        P[bn + "running_var"].copy_(rv[:C])
+        if (bn + "num_batches_tracked") in P:
+            P[bn + "num_batches_tracked"] += 1
+    return tables

@@ -151,8 +151,8 @@ int hg_spade_bwd_wgrad(const float* dout, const float* x, long x_bstride, const 
  *                          da1 [B,HW,128] (pixel-major); dp rows have stride dp_stride floats. */
 int hg_conv1x1_blocked(const float* x, int Cin, const void* wimg, const float* bias, float* out, int B, int Hg, int Wg,
                        int passes, void* stream);
-/* act (0 LeakyReLU/ReLU, 1 sine/cosine) selects the mask; ascale [B,256] scales g per (sample, channel) before the product
- * (K = 256 only); rk_* adds  sum_j rk_w[j][c]*rk_v[b][j][pixel]  (rk_w [3,256], rk_v [B,rk_n,HW], rk_n in 1..3) to the
+/* act (0 LeakyReLU/ReLU, 1 sine/cosine) selects the mask; ascale scales the operand per (sample, channel) before the
+ * product: [B,256] over g, or with g2 [B,512] (columns 0..255 scale g, 256..511 scale g2); rk_* adds  sum_j rk_w[j][c]*rk_v[b][j][pixel]  (rk_w [3,256], rk_v [B,rk_n,HW], rk_n in 1..3) to the
  * product before the mask -- the sigma / rgb heads of the renderer (modulated.py:62-73) feed back that way. */
 int hg_conv1x1_blocked_bwd(const float* g, const float* g2, const float* aux, const float* mod, const void* wimg_t,
                            float* out, double* sums, int Cout, float slope, int pixel_major, int act, const float* ascale,

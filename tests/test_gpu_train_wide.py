@@ -1,0 +1,368 @@
+"""Training at hidden_dim 384 (MAP3DBN) and 420 (MAP3DBN512L): the zero-padded forward with a tape and its backward
+(modules/wide_train.py) against fp64 / fp32 autograd through the restated reference, from the data-gradient kernel's
+K = 512 operand scale up to `Trainer.iteration`."""
+import importlib
+
+import pytest
+import torch
+
+pytestmark = pytest.mark.gpu
+
+WIDTHS = [384, 420]
+
+
+def _blocked(t):
+    """[B,C,HW] -> tile-blocked [B,T,C,128]."""
+    B, Cc, HW = t.shape
+    T = (HW + 127) // 128
+    pad = torch.zeros(B, Cc, T * 128, dtype=t.dtype)
+    pad[:, :, :HW] = t
+    return pad.reshape(B, Cc, T, 128).permute(0, 2, 1, 3).contiguous()
+
+
+def _planar(t, HW):
+    B, T, Cc, _ = t.shape
+    return t.permute(0, 2, 1, 3).reshape(B, Cc, T * 128)[:, :, :HW]
+
+
+def _halves_planar(pair, C, HW):
+    """Two tile-blocked halves [B,T,256,128] -> [B,C,HW] (padded channels dropped)."""
+    return torch.cat([_planar(p, HW) for p in pair], 1)[:, :C]
+
+
+def _rel(a, b):
+    return ((a - b).norm() / b.norm()).item()
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# 1. kernel: operand scale over K = 512
+# ----------------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("act,K", [(0, 512), (1, 512), (1, 256)])
+def test_conv_bwd_operand_scale(act, K):
+    abi = importlib.import_module("3dhumangan_b200.abi")
+    B, Hg, Wg = 2, 16, 20
+    HW = Hg * Wg
+    g = torch.Generator().manual_seed(31 + act + K)
+    go = torch.randn(B, K, HW, generator=g)
+    aux = torch.randn(B, 256, HW, generator=g)
+    W = torch.randn(K, 256, generator=g) / 16                   # forward weight [K outputs, 256 inputs]
+    ascale = 1.0 + 0.5 * torch.randn(B, K, generator=g)
+    mod = torch.stack([1.0 + 0.5 * torch.randn(B, 256, generator=g), 0.5 * torch.randn(B, 256, generator=g)], dim=1)
+    dy = torch.einsum("oc,bop->bcp", W.double(), go.double() * ascale.double()[:, :, None])
+    rk_w = rk_v = None
+    if act == 1:                # rank-3 head term
+        rk_w = torch.randn(3, 256, generator=g)
+        rk_v = torch.randn(B, 3, HW, generator=g)
+        dy = dy + torch.einsum("jc,bjp->bcp", rk_w.double(), rk_v.double())
+    pre = aux.double() * mod[:, 0, :, None].double() + mod[:, 1, :, None].double()
+    ref = dy * (torch.cos(pre) if act == 1 else torch.where(pre > 0, 1.0, 0.2))
+    s1, s2 = ref.sum(2), (ref * aux.double()).sum(2)
+
+    wimg_t, _ = abi.pack_weight(W.t().contiguous().cuda(), Nb=256)
+    gb = _blocked(go).cuda()
+    out = torch.full((B, gb.shape[1], 256, 128), float("nan"), device="cuda")
+    sums = torch.zeros(B, 2, 256, dtype=torch.float64, device="cuda")
+    abi.conv1x1_blocked_bwd(gb[:, :, :256].contiguous(), _blocked(aux).cuda(), wimg_t, out, sums,
+                            g2=gb[:, :, 256:].contiguous() if K == 512 else None, mod=mod.cuda(), act=act,
+                            ascale=ascale.cuda().contiguous(), rk_w=None if rk_w is None else rk_w.cuda(),
+                            rk_v=None if rk_v is None else rk_v.cuda(), B=B, Hg=Hg, Wg=Wg)
+    torch.cuda.synchronize()
+    got = _planar(out, HW).cpu().double()
+    safe = pre.abs() > 1e-5 if act == 0 else torch.ones_like(pre, dtype=torch.bool)
+    assert ((got - ref) * safe).abs().max() / ref.abs().max() < 5e-5
+    assert (sums[:, 0].cpu() - s1).abs().max() / s1.abs().max() < 5e-4
+    assert (sums[:, 1].cpu() - s2).abs().max() / s2.abs().max() < 5e-4
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# 2. renderer
+# ----------------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("C", WIDTHS)
+def test_render_wide_forward_and_backward(port, monkeypatch, C):
+    pkg = importlib.import_module("3dhumangan_b200")
+    rt = importlib.import_module("3dhumangan_b200.modules.render_train")
+    wo = importlib.import_module("3dhumangan_b200.modules.wide_ops")
+    wt = importlib.import_module("3dhumangan_b200.modules.wide_train")
+    B, R, S, seed = 2, 8, 32, 11
+    cfg = pkg.configs.baseline_config("tiny")
+    cfg.update(hidden_dim=C, feature_dim=C, num_steps=S, nerf_noise=0.5, white_back=True, last_back=False, clamp_mode="relu")
+    params = port.init_generator_params(cfg, seed=seed, sigma_gain=60.0, sigma_bias=2.0)
+    names = [n for n in params if n.startswith("neural_field.")]
+    g = torch.Generator().manual_seed(seed + 1)
+    N = R * S
+    pts = torch.rand(B, N, 3, generator=g) * 2 - 1
+    geo = torch.rand(B, N, 31, generator=g)
+    z = (torch.rand(B, R, S, generator=g) * 0.02 + 0.03).cumsum(-1) + 8.0
+    freq = torch.randn(B, 4 * C, generator=g)
+    phase = torch.randn(B, 4 * C, generator=g)
+    noise = torch.randn(B, R, S, 1, generator=g)
+    wgt = torch.randn(B, R, 3 + C, generator=g)
+
+    pg = {n: params[n].clone().cuda().requires_grad_(True) for n in names}
+    rec = torch.cat([pts, geo], -1).cuda()
+    monkeypatch.setattr(rt, "geo_records", lambda *a, **k: (rec, z.reshape(B, N).cuda().contiguous()))
+    tape = {}
+    feats, rgb01, _ = wo.render_forward_wide(pg, freq.cuda(), phase.cuda(), None, cfg, None, noise.cuda(), tape=tape)
+    dfq, dph = wt.render_backward_wide(tape, wgt[..., 3:].cuda(), wgt[..., :3].cuda())
+    torch.cuda.synchronize()
+
+    def oracle(mask):
+        pc = {n: params[n].clone().double().requires_grad_(True) for n in names}
+        fq, ph = freq.clone().double().requires_grad_(True), phase.clone().double().requires_grad_(True)
+        dirs = torch.zeros(B, N, 3, dtype=torch.float64)
+        dirs[..., -1] = -1
+        raw = port.siren(pc, pts.double(), fq, ph, geo.double(), dirs, 1.0, C, 4)
+        with monkeypatch.context() as mp:
+            if mask is not None:      # the sigma ReLU mask of the kernels (the gradient is discontinuous in it)
+                mp.setattr(port.F, "relu", lambda v: v * mask)
+            rgbf, _, _ = port.ray_integration(raw.reshape(B, R, S, -1), z.double()[..., None], noise.double(), cfg["nerf_noise"],
+                                              True, False, "relu")
+        return rgbf, pc, fq, ph
+
+    with torch.no_grad():
+        rgbf = oracle(None)[0]
+    assert (feats.cpu().double() - rgbf[..., 3:]).abs().max() / rgbf[..., 3:].abs().max() < 1e-3
+    assert (rgb01.cpu().double() - rgbf[..., :3]).abs().max() < 1e-3
+
+    mask = ((tape["sig"].cpu().double().reshape(B, R, S, 1) + noise.double() * cfg["nerf_noise"]) > 0).double()
+    assert 0.05 < mask.mean().item() < 0.95
+    rgbf, pc, fq, ph = oracle(mask)
+    (rgbf * wgt.double()).sum().backward()
+    bad = {}
+    for n in names:
+        assert pg[n].grad is not None and pg[n].grad.shape == pg[n].shape, n
+        e = _rel(pg[n].grad.cpu().double(), pc[n].grad)
+        if e > 1e-3:
+            bad[n] = e
+    assert not bad, sorted(bad.items(), key=lambda t: -t[1])
+    assert _rel(dfq.cpu().double(), fq.grad) < 1e-3
+    assert _rel(dph.cpu().double(), ph.grad) < 1e-3
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# 3. synthesis network
+# ----------------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("C,mode,mod_blocks", [(384, "mixed", [0, 1, 2]), (420, "isolated", [0, 1, 2])])
+def test_synthesis_wide_backward(port, monkeypatch, C, mode, mod_blocks):
+    """As tests/test_gpu_synthesis_bwd.py::_network_case: the fp64 reference is evaluated with the LeakyReLU / ReLU masks
+    the kernels differentiate through; the forward is compared without help."""
+    import torch.nn.functional as TF
+    pkg = importlib.import_module("3dhumangan_b200")
+    st = importlib.import_module("3dhumangan_b200.modules.synthesis_train")
+    wo = importlib.import_module("3dhumangan_b200.modules.wide_ops")
+    wt = importlib.import_module("3dhumangan_b200.modules.wide_train")
+    Rh, Rw, seed = 5, 7, 7
+    cfg = pkg.configs.baseline_config("tiny")
+    cfg.update(hidden_dim=C, feature_dim=C, gen_height=16, gen_width=24, render_height=Rh, render_width=Rw, mod_blocks=mod_blocks,
+               map3d_mode=mode)
+    B, Hg, Wg = 2, 16, 24
+    HW = Hg * Wg
+    params = port.init_generator_params(cfg, seed=seed)
+    names = [n for n in params if n.startswith(("synthesis_network.", "synthesis_input."))]
+    learn = [n for n in names if not n.endswith(("weight_u", "weight_v", "running_mean", "running_var", "num_batches_tracked"))]
+    g = torch.Generator().manual_seed(seed + 1)
+    fixed = torch.randn(B, 1, C, generator=g) * 0.5
+    fmap = torch.randn(B, C, Rh, Rw, generator=g) * 0.7
+    wgt = torch.randn(B, 3, Hg, Wg, generator=g)
+
+    pg = {n: params[n].clone().cuda() for n in names}
+    for n in learn:
+        pg[n].requires_grad_(True)
+    feat_lr = fmap.permute(0, 2, 3, 1).reshape(B, Rh * Rw, C).contiguous().cuda()
+    tape = st.SynthesisTape()
+    rgb = wo.synthesis_forward_wide(pg, feat_lr, fixed.cuda(), cfg, training=True, tape=tape)
+    tape.keep_masks = True
+    dfs, dfeat = wt.synthesis_backward_wide(pg, tape, wgt.cuda())
+    torch.cuda.synchronize()
+    masks, relu_masks = [], []
+    for rec in tape.halves:
+        if rec["pixel"]:
+            mk = _halves_planar(rec["mask"], C, HW).cpu()
+            masks.append(torch.where(mk, 1.0, 0.2).double().reshape(B, C, Hg, Wg))
+            relu_masks.append(_planar(rec["mask_a1"], HW).cpu().double().reshape(B, 128, Hg, Wg))
+            continue
+        relu_masks.append(None)
+        xp = _halves_planar(rec["x"], C, HW).double().cpu()
+        m = torch.cat(rec["mod_d"], -1)[..., :C].double().cpu()
+        pre = xp * m[:, 0, :, None] + m[:, 1, :, None]
+        masks.append(torch.where(pre > 0, 1.0, 0.2).reshape(B, C, Hg, Wg))
+
+    def oracle(mask_list):
+        pc = {n: (params[n].clone().double() if params[n].is_floating_point() else params[n].clone()) for n in names}
+        for n in learn:
+            pc[n].requires_grad_(True)
+        fc = fixed.clone().double().requires_grad_(True)
+        fm = fmap.clone().double().requires_grad_(True)
+        ii, jj = torch.linspace(-1, 1, Hg).double(), torch.linspace(-1, 1, Wg).double()
+        coords = torch.stack([ii[:, None].expand(Hg, Wg), jj[None, :].expand(Hg, Wg)], 0)[None].repeat(B, 1, 1, 1)
+        x0 = torch.sin(TF.conv2d(coords, pc["synthesis_input.network.0.weight"], pc["synthesis_input.network.0.bias"]))
+        style = TF.interpolate(fm, (Hg, Wg), mode="bilinear")
+        with monkeypatch.context() as mp:
+            if mask_list is not None:
+                it = iter(mask_list)
+                mp.setattr(port.F, "leaky_relu", lambda v, slope: v * next(it))
+                rit, real_relu = iter(relu_masks), TF.relu
+
+                def relu(v):
+                    mk = next(rit)
+                    return real_relu(v) if mk is None else v * mk
+                mp.setattr(port.F, "relu", relu)
+            out = port.synthesis_network(pc, x0, style, fc, cfg, training=True)
+        return out, pc, fc, fm
+
+    with torch.no_grad():
+        rgb_plain = oracle(None)[0]
+    assert (rgb.cpu().double() - rgb_plain).abs().max() / rgb_plain.abs().max() < 2e-4
+    rgb_ref, pc, fc, fm = oracle(masks)
+    (rgb_ref * wgt.double()).sum().backward()
+    scale = max(pc[n].grad.norm().item() for n in learn if pc[n].grad is not None)
+    bad = {}
+    for n in learn:
+        if pc[n].grad is None:         # the ToRGB layers of blocks 0-2, which the forward never uses
+            assert pg[n].grad is None or float(pg[n].grad.abs().max()) == 0.0, n
+            continue
+        assert pg[n].grad is not None and pg[n].grad.shape == pg[n].shape, n
+        a, b = pg[n].grad.cpu().double(), pc[n].grad.double()
+        err = a.norm().item() / scale if b.norm().item() < 1e-9 * scale else _rel(a, b)
+        if err > 5e-4:
+            bad[n] = err
+    assert not bad, sorted(bad.items(), key=lambda t: -t[1])[:8]
+    assert _rel(dfs.cpu().double().reshape(-1), fc.grad.reshape(-1)) < 5e-4
+    assert _rel(dfeat.cpu().double(), fm.grad.permute(0, 2, 3, 1).reshape(B, Rh * Rw, C)) < 5e-4
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# 4. whole generator
+# ----------------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("C,mode,legacy", [(384, "mixed", False), (420, "isolated", True)])
+def test_generator_wide_backward_matches_oracle(port, monkeypatch, C, mode, legacy):
+    """As tests/test_gpu_generator.py::test_generator_backward_matches_oracle_autograd, with its perturbation control."""
+    gen = importlib.import_module("3dhumangan_b200.modules.generator")
+    pkg = importlib.import_module("3dhumangan_b200")
+    rng = importlib.import_module("3dhumangan_b200.rng")
+    cfg = pkg.configs.baseline_config("tiny")
+    cfg.update(hidden_dim=C, feature_dim=C, map3d_mode=mode, legacy_mode=legacy, gen_height=16, gen_width=16, render_height=4,
+               render_width=4, num_steps=32, nerf_noise=0.0)
+    B = 2
+    params = port.init_generator_params(cfg, seed=21, sigma_gain=200.0, sigma_bias=1.0)
+
+    def make():
+        G = gen.Map3DGenerator(**cfg).cuda()
+        G.load_state_dict(params, strict=True)
+        G.train()
+        G.set_device(torch.device("cuda:0"))
+        return G
+
+    G = make()
+    cond = pkg.synthetic.make_conditions(B, seed=22)
+    cg = {k: v.cuda() for k, v in cond.items()}
+    z = torch.randn(B, cfg["latent_dim"], generator=torch.Generator().manual_seed(23))
+    wgt = torch.randn(B, 3, 16, 16, generator=torch.Generator().manual_seed(24))
+    wgt_r = torch.randn(B, 3, 4, 4, generator=torch.Generator().manual_seed(25))
+    torch.manual_seed(3)
+    u, noise = rng.draw_render_noise(B, 16, 32, "cpu", cfg["sample_dist"])
+    monkeypatch.setattr(rng, "draw_render_noise", lambda *a, **k: (u.cuda(), noise.cuda()))
+    out = G(z.cuda(), cg, **cfg)
+    assert out["rgbs"].requires_grad and out["rgbs_render"].requires_grad
+    ((out["rgbs"] * wgt.cuda()).sum() + (out["rgbs_render"] * wgt_r.cuda()).sum()).backward()
+    with torch.no_grad():
+        out_ng = make()(z.cuda(), cg, **cfg)
+    torch.cuda.synchronize()
+    assert _rel(out["rgbs"].detach().cpu(), out_ng["rgbs"].cpu()) < 1e-4
+    assert _rel(out["rgbs_render"].detach().cpu(), out_ng["rgbs_render"].cpu()) < 1e-4
+    for n, p in G.named_parameters():
+        assert p.grad is None or p.grad.shape == p.shape, n
+
+    pc = {n: (v.clone().requires_grad_(True) if v.is_floating_point() else v.clone()) for n, v in params.items()}
+    ref = port.generator_forward(pc, z, cond, cfg, u, noise, training=True)
+    assert (out["rgbs"].detach().cpu() - ref["rgbs"].detach()).abs().max() / ref["rgbs"].abs().max() < 1e-3
+    ((ref["rgbs"] * wgt).sum() + (ref["rgbs_render"] * wgt_r).sum()).backward()
+    worst = {}
+    for n, p in G.named_parameters():
+        if n not in pc or pc[n].grad is None or pc[n].grad.norm() == 0:
+            continue
+        assert p.grad is not None, n
+        worst[n] = ((p.grad.cpu().double() - pc[n].grad).norm() / pc[n].grad.norm()).item()
+    assert len(worst) > 100
+    top = max(v.grad.norm() for v in pc.values() if v.grad is not None)
+    over = {n: e for n, e in worst.items() if e > 0.1 and pc[n].grad.norm() > 1e-6 * top}
+    med = sorted(worst.values())[len(worst) // 2]
+    # control: the oracle's own gradient change under a perturbation of its forward as large as the kernels' forward error
+    fwd_err = float((out["rgbs"].detach().cpu() - ref["rgbs"].detach()).norm() / ref["rgbs"].detach().norm())
+    eps = max(fwd_err, 1e-6) / 8.0
+    gen_n = torch.Generator().manual_seed(99)
+    orig_half = port.spade_half
+    port.spade_half = lambda *a_, **k_: (lambda o: o * (1 + eps * torch.randn(o.shape, generator=gen_n)))(orig_half(*a_, **k_))
+    try:
+        pp = {n: (v.clone().requires_grad_(True) if v.is_floating_point() else v.clone()) for n, v in params.items()}
+        refp = port.generator_forward(pp, z, cond, cfg, u, noise, training=True)
+    finally:
+        port.spade_half = orig_half
+    ((refp["rgbs"] * wgt).sum() + (refp["rgbs_render"] * wgt_r).sum()).backward()
+    ctrl_of = {n: float((pp[n].grad - pc[n].grad).norm() / pc[n].grad.norm()) for n in worst if pp[n].grad is not None}
+    ctrl = sorted(ctrl_of.values())
+    med_ctrl = ctrl[len(ctrl) // 2]
+    print(f"hidden {C}: kernels vs oracle median {med:.2e} (forward error {fwd_err:.2e}); control median {med_ctrl:.2e}; "
+          f"over 0.1: {[(n, round(e, 3), round(ctrl_of.get(n, 0.0), 3)) for n, e in over.items()]}")
+    # No parameter may be over 0.1, with one named exception: the sigma bias, whose gradient is the sum of dsig over every ray
+    # sample of the batch.  Its terms cancel, so the run-to-run differences of the synthesis backward (fp32 atomics in the
+    # batch statistics and weight gradients) that feed dsig move it far more than any other parameter: at 420 it measured
+    # 0.19 and 0.11 in two of five runs, and the control alone moved it by 0.09.  It must then stay within 4x of the control;
+    # test_render_wide_forward_and_backward pins its arithmetic to 1e-3 for a fixed dsig.
+    SUM_OVER_SAMPLES = "neural_field.sigma_layer.bias"
+    bad = {n: e for n, e in over.items() if n != SUM_OVER_SAMPLES or e > 4 * ctrl_of.get(n, 0.0)}
+    assert not bad, sorted(bad.items(), key=lambda t: -t[1])[:8]
+    assert med < 2e-2, (med, med_ctrl)
+    assert med < 4 * med_ctrl + 1e-3, (med, med_ctrl, fwd_err)
+
+
+def test_wide_surface_guards(port):
+    """last_back=True under autograd and widths above 512 still raise."""
+    gen = importlib.import_module("3dhumangan_b200.modules.generator")
+    pkg = importlib.import_module("3dhumangan_b200")
+    cfg = pkg.configs.baseline_config("tiny")
+    cfg.update(hidden_dim=384, feature_dim=384, gen_height=16, gen_width=16, render_height=4, render_width=4, last_back=True)
+    G = gen.Map3DGenerator(**cfg).cuda().train()
+    G.set_device(torch.device("cuda:0"))
+    cond = {k: v.cuda() for k, v in pkg.synthetic.make_conditions(2, seed=1).items()}
+    with pytest.raises(RuntimeError, match="last_back"):
+        G(torch.randn(2, cfg["latent_dim"], device="cuda"), cond, **cfg)
+    cfg.update(hidden_dim=640, feature_dim=640, last_back=False)
+    G = gen.Map3DGenerator(**cfg).cuda().train()
+    G.set_device(torch.device("cuda:0"))
+    with pytest.raises(RuntimeError, match="512"):
+        G(torch.randn(2, cfg["latent_dim"], device="cuda"), cond, **cfg)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# 5. trainer
+# ----------------------------------------------------------------------------------------------------------------------
+def test_trainer_map3dbn_amp(pkg):
+    """MAP3DBN (384) at small shapes: fp16 autocast + GradScaler, four iterations including a do_r1 phase."""
+    gen = importlib.import_module("3dhumangan_b200.modules.generator")
+    disc = importlib.import_module("3dhumangan_b200.modules.discriminator")
+    ts = importlib.import_module("3dhumangan_b200.train_step")
+    cfg = pkg.configs.baseline_config("C1")
+    assert cfg["hidden_dim"] == 384 and cfg["r1_lambda"] == 0.25
+    cfg.update(gen_height=128, gen_width=64, render_height=16, render_width=8, num_steps=32, nerf_noise=0.5)
+    B = 2
+    torch.manual_seed(0)
+    G = gen.Map3DGenerator(**cfg).cuda().train()
+    G.set_device(torch.device("cuda:0"))
+    D = disc.UNetDiscriminator(**cfg).cuda().train()
+    t = ts.Trainer(G, D, cfg, amp=True, ddp=False)
+    batch = dict(cond={k: v.cuda() for k, v in pkg.synthetic.make_conditions(B, seed=1).items()},
+                 images=torch.randn(B, 3, 128, 64, device="cuda").clamp_(-1, 1),
+                 labels=torch.randint(1, cfg["label_dim"], (B, 128, 64), device="cuda"))
+    g0 = {n: p.detach().clone() for n, p in G.named_parameters()}
+    for _ in range(4):                    # phases 0..3: the last one is a do_r1 phase
+        d, g_ = t.iteration(batch)
+        assert torch.isfinite(d) and torch.isfinite(g_)
+    torch.cuda.synchronize()
+    moved = [n for n, p in G.named_parameters() if not torch.equal(p.detach(), g0[n])]
+    for prefix in ("neural_field.", "synthesis_network.", "neural_field_mapping_network.", "synthesis_mapping_network."):
+        assert any(n.startswith(prefix) for n in moved), prefix
+    for p in list(G.parameters()) + list(D.parameters()):
+        assert torch.isfinite(p).all()
+    ptrs = [p.grad.untyped_storage().data_ptr() for p in G.parameters() if p.grad is not None]
+    assert len(ptrs) > 0 and len(ptrs) == len(set(ptrs))
