@@ -84,6 +84,9 @@ SIGNATURES = {
     "hg_smpl_shape": (c_int, [c_void_p] * 6 + [c_int] * 4 + [c_void_p]),
     "hg_smpl_pose": (c_int, [c_void_p, c_int, c_void_p, c_int] + [c_void_p] * 6 + [c_int, c_int, c_void_p]),
     "hg_smpl_skin": (c_int, [c_void_p, c_long, c_void_p, c_void_p, c_int, c_void_p, c_long, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "hg_raster_project": (c_int, [c_void_p, c_void_p, c_void_p, c_float, c_void_p, c_int, c_int, c_void_p]),
+    "hg_raster_faces": (c_int, [c_void_p, c_void_p] + [c_int] * 5 + [c_void_p, c_void_p]),
+    "hg_raster_resolve": (c_int, [c_void_p] * 5 + [c_int] * 5 + [c_void_p] * 6),
     "hg_spectral_entry_bytes": (c_int, []),
     "hg_spectral_norm": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_float, c_void_p]),
 }

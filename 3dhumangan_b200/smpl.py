@@ -52,6 +52,45 @@ class SMPLModel:
         return SMPLModel.from_arrays(v, torch.randn(V, 3, NB, generator=g) * 0.01, torch.randn((J - 1) * 9, V * 3, generator=g) * 0.01,
                                      jr, parents, w, device)
 
+    @staticmethod
+    def synthetic_surface(device="cuda", J=24, NB=10, seed=0):
+        """A stand-in with SMPL's mesh sizes for the rasteriser -> (model, faces [13776,3] int64).  The template is a closed
+        genus-0 surface (a 84-ring x 82-segment sphere plus two poles: 6 890 vertices, 13 776 = 2V - 4 faces)
+        shaped into an upright body with one raised arm on +x, so its silhouette is neither left-right nor up-down symmetric.
+        Skinning weights fall off smoothly with the distance to joints placed along the body, so posed meshes stay smooth."""
+        g = torch.Generator().manual_seed(seed)
+        rings, segs = 84, 82
+        th = torch.arange(1, rings + 1, dtype=torch.float64) * (math.pi / (rings + 1))
+        ph = torch.arange(segs, dtype=torch.float64) * (2 * math.pi / segs)
+        st, ct = torch.sin(th)[:, None], torch.cos(th)[:, None]
+        sp, cp = torch.sin(ph)[None], torch.cos(ph)[None]
+        yy = (0.85 * ct).expand(rings, segs)
+        arm = 0.35 * torch.exp(-((yy - 0.35) / 0.12) ** 2) * cp.clamp_min(0) ** 4           # +x only, above the waist
+        ring = torch.stack([(0.22 + arm) * st * cp, yy, 0.12 * st * sp], -1).reshape(-1, 3)
+        v = torch.cat([torch.tensor([[0.0, 0.85, 0.0]], dtype=torch.float64), ring, torch.tensor([[0.0, -0.85, 0.0]], dtype=torch.float64)])
+        idx = lambda r, s: 1 + r * segs + s % segs
+        faces = [(0, idx(0, s + 1), idx(0, s)) for s in range(segs)]
+        for r in range(rings - 1):
+            for s in range(segs):
+                a, b, c, d = idx(r, s), idx(r, s + 1), idx(r + 1, s), idx(r + 1, s + 1)
+                faces += [(a, b, c), (b, d, c)]
+        last = 1 + rings * segs
+        faces += [(last, idx(rings - 1, s), idx(rings - 1, s + 1)) for s in range(segs)]
+        faces = torch.tensor(faces, dtype=torch.int64)
+        parents = torch.tensor([-1] + [max(0, (i - 1) // 2) for i in range(1, J)], dtype=torch.int32)
+        anchors = torch.stack([0.1 * torch.sin(torch.arange(J, dtype=torch.float64)), torch.linspace(-0.7, 0.7, J, dtype=torch.float64),
+                               torch.zeros(J, dtype=torch.float64)], -1)
+        d2 = torch.cdist(v, anchors) ** 2
+        jr = torch.softmax(-d2.T / 0.01, 1)
+        w = torch.softmax(-d2 / 0.02, 1)
+        top = torch.topk(w, 4, dim=1)
+        w = torch.zeros_like(w).scatter_(1, top.indices, top.values)
+        w = w / w.sum(1, keepdim=True)
+        V = v.shape[0]
+        model = SMPLModel.from_arrays(v, torch.randn(V, 3, NB, generator=g, dtype=torch.float64) * 0.01,
+                                      torch.randn((J - 1) * 9, V * 3, generator=g, dtype=torch.float64) * 1e-3, jr, parents, w, device)
+        return model, faces.to(device)
+
 
 @torch.no_grad()
 def lbs(betas, pose, model: SMPLModel, pose2rot=True):
@@ -129,15 +168,22 @@ def _euler_xyz(e):
 
 
 @torch.no_grad()
-def cam2world_fix_body(cond, h_rotation, v_rotation, r_rotation):
-    """The view rotation of `SHHQPreprocessor._forward_fix_body` (preprocessor.py:72-98) -> cam2world [B,4,4]."""
-    R, T = cond["R"], cond["T"]
+def body_rotation(cond, h_rotation, v_rotation, r_rotation):
+    """The body rotation R of `SHHQPreprocessor._forward_fix_body` (preprocessor.py:82-87) -> [B,3,3]."""
+    R = cond["R"]
     B = R.shape[0]
     euler = torch.zeros(B, 3, dtype=torch.float32, device=R.device)
     euler[:, 1] = -torch.as_tensor(h_rotation, dtype=torch.float32, device=R.device)
     euler[:, 0] = math.pi - torch.as_tensor(v_rotation, dtype=torch.float32, device=R.device)
     euler[:, 2] = -torch.as_tensor(r_rotation, dtype=torch.float32, device=R.device)
-    Rb = cond["full_pose"][:, 0] @ _euler_xyz(euler)
+    return cond["full_pose"][:, 0] @ _euler_xyz(euler)
+
+
+@torch.no_grad()
+def cam2world_fix_body(cond, h_rotation, v_rotation, r_rotation):
+    """The view rotation of `SHHQPreprocessor._forward_fix_body` (preprocessor.py:72-98) -> cam2world [B,4,4]."""
+    R, T = cond["R"], cond["T"]
+    Rb = body_rotation(cond, h_rotation, v_rotation, r_rotation)
     body = F.pad(Rb, (0, 1, 0, 1))
     body[:, -1, -1] = 1.0
     return torch.inverse(torch.bmm(torch.bmm(R, T), body).float())

@@ -18,6 +18,7 @@ modules/discriminator_train.py).  Loss reduction, clipping, Adam and EMA are mul
 from __future__ import annotations
 
 import math
+import random
 
 import torch
 import torch.nn.functional as F
@@ -187,9 +188,14 @@ class Trainer:
     optional z_d / z_g latents (drawn like `z_sampler` otherwise)).  `meta` is the merged curriculum dict that the
     reference splats into every call."""
 
-    def __init__(self, G, D, meta, *, amp=None, ddp=None, amp_dtype=torch.float16, ema_decay=0.999, fused=True):
+    def __init__(self, G, D, meta, *, amp=None, ddp=None, amp_dtype=torch.float16, ema_decay=0.999, fused=True, preprocessor=None):
         """fused=True: the loss / clipping / Adam / EMA tail on the sm_90a kernels of csrc/trainer.cu (ops.trainer_ops);
-        fused=False: the same steps as torch calls (F.cross_entropy, clip_grad_norm_, torch.optim.Adam, foreach lerp)."""
+        fused=False: the same steps as torch calls (F.cross_entropy, clip_grad_norm_, torch.optim.Adam, foreach lerp).
+        preprocessor: a `preprocess.Preprocessor`.  With one, each step draws a view for `batch["cond"]` as
+        phase_trainer.py:305,329 do, and the segmentation targets follow :350-353 and :533 -- the rasterised map on rotate phases,
+        otherwise the rasterised map or `batch["labels"]` (the dataset's body_segments) with probability 1/2 each, drawn with
+        `random.random()`.  Without one, `batch["cond"]` is used as given and `batch["labels"]` is the target in every phase."""
+        self.preprocessor = preprocessor
         import torch.distributed as dist
         self.meta = dict(meta)
         self.fused = bool(fused)
@@ -261,6 +267,10 @@ class Trainer:
         self._check_phase(phase)
         self.optimizer_D.zero_grad()
         real_images, labels, cond = batch["images"], batch["labels"], batch["cond"]
+        if self.preprocessor is not None:
+            cond = self.preprocessor(dict(cond), phase["rotate"], **meta)
+            if phase["rotate"] or random.random() < 0.5:
+                labels = cond["rasterized_segments"]
         B = real_images.shape[0]
         with self._autocast():
             with torch.no_grad():
@@ -303,6 +313,8 @@ class Trainer:
         self._check_phase(phase)
         self.optimizer_G.zero_grad()
         real_images, labels, cond = batch["images"], batch["labels"], batch["cond"]
+        if self.preprocessor is not None:
+            cond = self.preprocessor(dict(cond), phase["rotate"], **meta)
         B = real_images.shape[0]
         z = self._z(batch, "z_g", B, real_images.device)
         split = B // self.batch_split
@@ -327,7 +339,10 @@ class Trainer:
                     gan_loss = gan_lambda * F.softplus(-pred_gen).mean() if gan_lambda > 0 else 0 * pred_gen.sum()
                     latent_loss = out["latents"].sum() * 0
                     if meta["segmentation_lambda"] > 0:
-                        seg = self._seg_loss(out["segments"], labels[sl]) * meta["segmentation_lambda"]
+                        gt = labels[sl]
+                        if self.preprocessor is not None and (phase["rotate"] or random.random() < 0.5):
+                            gt = sub["rasterized_segments"]
+                        seg = self._seg_loss(out["segments"], gt) * meta["segmentation_lambda"]
                     else:
                         seg = out["segments"].sum() * 0
                     g_loss = (gan_loss + latent_loss + seg) / self.batch_split

@@ -276,6 +276,22 @@ int hg_smpl_pose(const float* jpart, int nblk, const float* pose, int pose_is_ro
 int hg_smpl_skin(const float* v_in, long v_bstride, const float* feat, const float* posedirs, int P, const float* lbs_weights,
                  long w_bstride, const float* A, float* verts, int B, int V, int J, void* stream);
 
+/* ---- SMPL label maps: the segmentation targets (SURVEY.md 8f-2) -----------------------------------------------------------
+ * Replaces pytorch3d's MeshRasterizer in SHHQPreprocessor._forward_rasterize (lib/data/preprocessor.py:138-176): blur 0, one face
+ * per pixel, no culling, perspective-correct barycentrics; the restated contract is oracle/raster_port.py.  faces [F,3] int64 is
+ * shared by the batch.
+ * hg_raster_project: proj [B,V,3] = (f X/Z, f Y/Z, Z) with X_view = verts [B,V,3] @ R [B,3,3] + T [B,3] (row vectors).
+ * hg_raster_faces  : zkey [B,H,W] u64 (cleared by the call) = (float bits of pz) << 32 | face of the nearest covering face,
+ *                    lowest face on equal pz; ~0 = background.
+ * hg_raster_resolve: segments [B,H,W] int64 = faces_to_labels[face] + 2 (1 = background); semantics [B,3,H,W] = tpose0 [V,3] at
+ *                    the face vertex with the first largest barycentric (0 = background); pix_to_face [B,H,W] int64 (b*F + face
+ *                    or -1), zbuf [B,H,W] and bary [B,H,W,3] (-1 on background) are optional (NULL). */
+int hg_raster_project(const float* verts, const float* R, const float* T, float focal, float* proj, int B, int V, void* stream);
+int hg_raster_faces(const float* proj, const long long* faces, int B, int V, int F, int H, int W, unsigned long long* zkey, void* stream);
+int hg_raster_resolve(const float* proj, const long long* faces, const long long* faces_to_labels, const float* tpose0,
+                      const unsigned long long* zkey, int B, int V, int F, int H, int W, long long* segments, float* semantics,
+                      long long* pix_to_face, float* zbuf, float* bary, void* stream);
+
 /* ---- loss + optimiser tail of a training iteration (SURVEY.md 8f-1) ---------------------------------------------------
  * Class-balanced segmentation cross entropy, PhaseTrainer._calculate_segmentation_loss mode 'cross_entropy_balanced'
  * (lib/trainers/phase_trainer.py:203-256): histogram of the int64 labels -> per-class coefficients (numel / (occ * n_occ) *
