@@ -15,6 +15,7 @@ namespace hg {
 
 constexpr int kDwThreads = 256;   // two warpgroups: operands, wgmma, drain
 constexpr int kDwCo = 128;        // output channels per work item of the whole-layer mode
+constexpr int kDwMaxTiles = 64;   // whole-layer mode: 128-pixel tiles summed by one CTA (bounds the fp32 accumulation)
 constexpr uint32_t kDwImg = 256 * 128;
 constexpr uint32_t kDwSmemBytes = 4 * kDwImg + 8 * 8 + 16 + 1024;
 
@@ -353,6 +354,11 @@ static void wgrad_layer_geometry(int B, int H, int W, int Cout, int Cin, int ksi
   // grid is many small items of different cost
   int g = *nitems == 1 ? hg::num_sms() : 4 * hg::num_sms() / *nitems;
   if (g < 1) g = 1;
+  // at most kDwMaxTiles tiles per CTA: each CTA sums its tiles in fp32 wgmma accumulators before the fp64 reduction, and the
+  // bf16x3 product's error grows with that length (a 3x3 256 -> 64 layer at 512x512, B = 4, measured 6.3e-5 relative L2 with
+  // 141 tiles per CTA, 3.2e-5 with 70)
+  const int cap = (B * ((H * W + 127) / 128) + hg::kDwMaxTiles - 1) / hg::kDwMaxTiles;
+  if (g < cap) g = cap;
   *gx = tiles < g ? tiles : g;
   *item_stride = static_cast<long>(*gx) * *per * 256 * nq_max;
 }
