@@ -276,11 +276,16 @@ def spade_conv(x, x_bstride, wimg, bias, out, *, B, Hg, Wg, mod=None, scsh=None,
                wgb=None, bgb=None, skip=None, stats=None, rgb_w=None, rgb_b=None, rgb_in=None, rgb_out=None,
                Rh=0, Rw=0, passes=3):
     """One SPADE half-block (see csrc/synth.cu).  All tensors fp32 CUDA; `stats` is a float64 view [>=512]."""
+    tag = None
+    if TIMING_TAGS:
+        flags = "".join(f" {n}" for n, t in (("skip", skip), ("rgb", rgb_w), ("stats", stats)) if t is not None)
+        flags += " xshared" if x_bstride == 0 else ""
+        tag = f"{'pixel' if p_lr is not None else 'const'}{flags} {Hg}x{Wg} B{B}"
     with torch.cuda.device_of(out):
         call("hg_spade_conv", ptr(x), int(x_bstride), ptr(mod), ptr(scsh), ptr(p_lr), int(p_stride), ptr(p_bias),
                                   ptr(wgb), ptr(bgb), ptr(wimg), ptr(bias), ptr(skip), ptr(out), ptr(stats),
                                   ptr(rgb_w), ptr(rgb_b), ptr(rgb_in), ptr(rgb_out), B, 256, Hg, Wg, Rh, Rw, passes,
-                                  stream())
+                                  stream(), tag=tag)
     return out
 
 
