@@ -13,18 +13,21 @@ synthesis network; a "pixel" is a sample point p = ray*S + s) and keeps the 8 li
     sigma, rgb_pre                                               hg_render_heads
     ray_out = composite(...)                                     hg_render_composite
 
-Backward: hg_render_composite_bwd, hg_render_heads_bwd, then per layer the blocked data-gradient kernel with the
-cosine mask (the sigma / rgb heads enter as rank-1 / rank-3 terms of its epilogue, the FiLM frequency of the consumer
-as a per-(sample, channel) scale of its operand) and the blocked weight-gradient kernel with the sine operand.
-d freq / d phase come from the per-(b,c) sums S1 = sum dpre, S2 = sum dpre*x of the data-gradient kernels through
-torch autograd on the [B,256] tables.  Geometry features carry no gradient (wrapped in no_grad in the reference,
-map3d_generator.py:196-205).
+Backward (`mlp_backward`, one for every width): the tape holds each activation as nh 256-channel halves -- nh = 1 here,
+nh = 2 from the zero-padded forward of modules/wide_ops.py at hidden_dim 384 / 420.  Per feature half
+hg_render_composite_bwd and hg_render_heads_bwd, then per layer and input half the blocked data-gradient kernel with
+the cosine mask (K = nh*256 from the output-half gradients; the sigma / rgb heads enter as rank-1 / rank-3 terms of
+its epilogue, the FiLM frequency of the consumer as a per-(sample, channel) scale of its operand) and per (output
+half, input half) the blocked weight-gradient kernel with the sine operand.  d freq / d phase come from the per-(b,c)
+sums S1 = sum dpre, S2 = sum dpre*x of the data-gradient kernels through torch autograd on the [B,256] tables.
+Geometry features carry no gradient (wrapped in no_grad in the reference, map3d_generator.py:196-205).
 """
 from __future__ import annotations
 
 import torch
 
 from .. import abi
+from .wide_ops import _pad2
 
 H = 256
 
@@ -60,9 +63,9 @@ def mlp_forward_train(P, freq, phase, rec, z_vals, noise, cfg, *, geo_dim=31, lo
     fq = freq.detach().float().requires_grad_(True)
     ph = phase.detach().float().requires_grad_(True)
     f = fq * 15 + 30
-    mods = [torch.stack([f[:, i * H:(i + 1) * H], ph[:, i * H:(i + 1) * H]], dim=1) for i in range(4)]      # [B,2,256] each
+    mods_h = [torch.stack([f[:, i * H:(i + 1) * H], ph[:, i * H:(i + 1) * H]], dim=1) for i in range(4)]    # [B,2,256] each
     mod30 = torch.stack([torch.full((B, H), 30.0, **f32), torch.zeros(B, H, **f32)], dim=1).contiguous()
-    mods_d = [m.detach().contiguous() for m in mods]
+    mods = [m.detach().contiguous() for m in mods_h]
 
     rec_b = blocked_points(rec[..., :3 + geo_dim], 128)
     Wa = torch.zeros(H, 128, **f32)
@@ -75,116 +78,155 @@ def mlp_forward_train(P, freq, phase, rec, z_vals, noise, cfg, *, geo_dim=31, lo
     outs = [abi.act_conv1x1_blocked(lin_a, mod30, pack(g("network.0.layer.weight")), g("network.0.layer.bias").detach(), new(),
                                     x2=lin_b, **kw)]
     for i in range(1, 4):
-        outs.append(abi.act_conv1x1_blocked(outs[-1], mods_d[i - 1], pack(g(f"network.{i}.layer.weight")),
+        outs.append(abi.act_conv1x1_blocked(outs[-1], mods[i - 1], pack(g(f"network.{i}.layer.weight")),
                                             g(f"network.{i}.layer.bias").detach(), new(), **kw))
     wcol = g("color_layer_sine.layer.weight")
     dvec = torch.tensor(locked_dir, **f32)
     bcol = g("color_layer_sine.layer.bias") + wcol[:, :3] @ dvec            # autograd: bias and the direction columns
-    lin_c = abi.act_conv1x1_blocked(outs[3], mods_d[3], pack(wcol[:, 3:]), bcol.detach().contiguous(), new(), **kw)
-    feat = abi.act_conv1x1_blocked(lin_c, mods_d[3], pack(g("feature_layer_linear.weight")),
+    lin_c = abi.act_conv1x1_blocked(outs[3], mods[3], pack(wcol[:, 3:]), bcol.detach().contiguous(), new(), **kw)
+    feat = abi.act_conv1x1_blocked(lin_c, mods[3], pack(g("feature_layer_linear.weight")),
                                    g("feature_layer_linear.bias").detach(), new(), **kw)
     w_sigma = g("sigma_layer.weight").detach().reshape(-1).float().contiguous()
     w_rgb = g("color_layer_linear.weight").detach().float().contiguous()
     heads_b = torch.cat([g("sigma_layer.bias").detach().reshape(1), g("color_layer_linear.bias").detach().reshape(3)]).float().contiguous()
-    sig, rgbp = abi.render_heads(outs[3], lin_c, mods_d[3], w_sigma, w_rgb, heads_b, B=B, N=N)
+    sig, rgbp = abi.render_heads(outs[3], lin_c, mods[3], w_sigma, w_rgb, heads_b, B=B, N=N)
     noise = None if noise is None else noise.reshape(B, N).float().contiguous()
     comp = dict(B=B, R=R, S=S, noise_std=cfg["nerf_noise"], white_back=cfg.get("white_back", False),
                 softplus=cfg["clamp_mode"] == "softplus")
-    ray_out, w = abi.render_composite(sig, z_vals, noise, rgbp, feat, **comp)
-    tape = dict(P=P, prefix=prefix, geo_dim=geo_dim, fq=fq, ph=ph, mods=mods, mods_d=mods_d, mod30=mod30, rec_b=rec_b,
-                lin_a=lin_a, lin_b=lin_b, outs=outs, lin_c=lin_c, feat=feat, sig=sig, rgbp=rgbp, z=z_vals, noise=noise, comp=comp,
-                kw=kw, bcol=bcol, w_sigma=w_sigma, w_rgb=w_rgb, B=B, N=N, weights=w)
+    ray_out, _ = abi.render_composite(sig, z_vals, noise, rgbp, feat, **comp)
+    tape = dict(P=P, prefix=prefix, C=H, Fd=H, geo_dim=geo_dim, fq=fq, ph=ph, mods=[(m,) for m in mods], mods_h=[(m,) for m in mods_h],
+                m30=(mod30,), rec_b=rec_b, lin_a=(lin_a,), lin_b=(lin_b,), outs=[(o,) for o in outs], lin_c=(lin_c,), feat=(feat,),
+                sig=sig, rgbp=rgbp, z=z_vals, noise=noise, comp=comp, kw=kw, bcol=bcol, w_sigma=w_sigma, w_rgb=w_rgb, B=B, N=N)
     return ray_out, tape
 
 
-def mlp_backward(tape, dray, grads=None):
-    """dray [B,R,260] (gradient w.r.t. feat | rgb | depth; the depth column is ignored, as no loss uses it).
-    Adds the gradients of the neural-field parameters to `grads` (name -> tensor; to `.grad` when grads is None) and
-    returns (d freq, d phase) [B,4*256] each."""
-    from .synthesis_train import grad_accumulator
+def mlp_backward(tape, dfeat, drgb, grads=None):
+    """Backward of the training renderer at every width.  dfeat [B,R,Fd] and drgb [B,R,3] (either may be None) are the
+    gradients w.r.t. the ray features and rgb.  Adds the gradients of the neural-field parameters to `grads` (name ->
+    tensor; to `.grad` when grads is None) and returns (d freq, d phase) [B,4*C] each.
+
+    The tape is the dict `mlp_forward_train` (hidden_dim 256) or `wide_ops.render_forward_wide(..., tape=tape)` (the
+    zero-padded widths) fills.  Every point activation is a tuple of nh tile-blocked halves [B,T,256,128], nh = 1 at
+    256 and 2 at the padded widths:
+        lin_a, lin_b, outs[0..3], lin_c, feat   the linear outputs
+        mods[0..3], m30     the detached FiLM tables (f, phi) [B,2,256] per half; m30 = (30, 0) of the first layers
+        mods_h[0..3]        the same tables with autograd history from the leaves fq, ph
+    and w_sigma [nh*256], w_rgb [3,nh*256] zero-padded, bcol (colour bias + direction columns) with history, the
+    compositing inputs sig, rgbp, z, noise, comp, and rec_b, C, Fd, geo_dim, B, N, kw, P, prefix.  Padded channels
+    carry zero weights and zero FiLM tables, so their gradients are zero up to the trimming to each parameter's shape."""
+    from .synthesis_train import _packT, grad_accumulator
     P, prefix = tape["P"], tape["prefix"]
     g = lambda n: P[prefix + n]
     acc_ = grad_accumulator(P, grads)
-    acc = lambda n, grad: acc_(prefix + n, grad)
-    B, N, kw = tape["B"], tape["N"], tape["kw"]
-    dev = dray.device
+    acc = lambda n, gr: acc_(prefix + n, gr)
+    B, N, C, Fd, kw = tape["B"], tape["N"], tape["C"], tape["Fd"], tape["kw"]
+    mods, m30, outs, lin_c = tape["mods"], tape["m30"], tape["outs"], tape["lin_c"]
+    nh = len(lin_c)
+    halves = range(nh)
+    W = nh * H
+    sl = lambda h: slice(h * H, (h + 1) * H)
+    dev = tape["sig"].device
     f32 = dict(dtype=torch.float32, device=dev)
     T = N // 128
     full = T * H * 128
     new = lambda: torch.empty(B, T, H, 128, **f32)
-    packT = lambda w: abi.pack_weight(w.detach().float().t().contiguous(), Nb=256)[0]
-    mods_d, mod30, outs = tape["mods_d"], tape["mod30"], tape["outs"]
+    scale = lambda m: torch.cat([t[:, 0] for t in m], -1).contiguous()        # FiLM frequency [B,nh*256] of a consumer
+    pscale = lambda m: [t[:, 0].contiguous() for t in m]
 
-    dfeat, drgbp, dsig = abi.render_composite_bwd(tape["sig"], tape["z"], tape["noise"], tape["rgbp"], tape["feat"],
-                                                  dray.float().contiguous(), **tape["comp"])
-    hb = abi.render_heads_bwd(outs[3], tape["lin_c"], mods_d[3], dsig, drgbp, B=B, N=N)
-    acc("sigma_layer.weight", hb[:H].float())
-    acc("color_layer_linear.weight", hb[H:4 * H].float().reshape(3, H))
-    acc("sigma_layer.bias", hb[4 * H:4 * H + 1].float())
-    acc("color_layer_linear.bias", hb[4 * H + 1:].float())
+    # ---- compositing per feature half: the rgb gradient enters once; dsig is linear in dray, so the halves' terms add
+    dfh, drgbp, dsig = [], None, None
+    for h in halves:
+        dray = torch.zeros(B, tape["comp"]["R"], 260, **f32)
+        if dfeat is not None:
+            part = dfeat[..., sl(h)]
+            dray[..., :part.shape[-1]] = part
+        if h == 0 and drgb is not None:
+            dray[..., 256:259] = drgb
+        df, dp, ds = abi.render_composite_bwd(tape["sig"], tape["z"], tape["noise"], tape["rgbp"], tape["feat"][h], dray, **tape["comp"])
+        dfh.append(df)
+        drgbp = dp if h == 0 else drgbp
+        dsig = ds if dsig is None else dsig + ds
+        del dray
+    # ---- heads (the biases once)
+    hb = [abi.render_heads_bwd(outs[3][h], lin_c[h], mods[3][h], dsig, drgbp, B=B, N=N) for h in halves]
+    acc("sigma_layer.weight", torch.cat([t[:H] for t in hb])[:C].float())
+    acc("color_layer_linear.weight", torch.cat([t[H:4 * H].reshape(3, H) for t in hb], -1)[:, :C].float())
+    acc("sigma_layer.bias", hb[0][4 * H:4 * H + 1].float())
+    acc("color_layer_linear.bias", hb[0][4 * H + 1:].float())
 
-    dmods = [torch.zeros(B, 2, H, **f32) for _ in range(4)]
-    sums = lambda: torch.zeros(B, 2, H, dtype=torch.float64, device=dev)
+    dmods = [[torch.zeros(B, 2, H, **f32) for _ in halves] for _ in range(4)]
 
-    def add_film(i, s):          # d g1 = sum dpre*x, d g0 = sum dpre
-        dmods[i] += torch.stack([s[:, 1], s[:, 0]], dim=1).float()
+    def dgrad(gs, xs, Wp, mods_in, film=None, ascale=None, rk_w=None, rk_v=None):
+        """Data gradient of one zero-padded layer per input half, K = nh*256 from the output halves' gradients gs; its
+        S1 / S2 sums go to FiLM slice `film`."""
+        res = []
+        for ih in halves:
+            s = torch.zeros(B, 2, H, dtype=torch.float64, device=dev)
+            res.append(abi.conv1x1_blocked_bwd(gs[0], xs[ih], _packT(Wp, ih), new(), s, g2=gs[1] if nh == 2 else None, mod=mods_in[ih],
+                                               act=1, ascale=ascale, rk_w=None if rk_w is None else rk_w[:, sl(ih)].contiguous(),
+                                               rk_v=rk_v, **kw))
+            if film is not None:        # d g1 = sum dpre*x, d g0 = sum dpre
+                dmods[film][ih] += torch.stack([s[:, 1], s[:, 0]], dim=1).float()
+        return tuple(res)
 
-    rk3 = tape["w_rgb"]                                                        # [3,256]
-    rk1 = torch.zeros(3, H, **f32)
+    def wgrad(gs, xs, mods_in, ps):
+        """[nh*256, nh*256] weight gradient block by block, [nh*256] bias gradient."""
+        dW = torch.empty(W, W, **f32)
+        dbs = []
+        for oh in halves:
+            for ih in halves:
+                dw, db = abi.act_wgrad_blocked(gs[oh], xs[ih], full, mods_in[ih], act=1, pscale=None if ps is None else ps[oh], **kw)
+                dW[sl(oh), sl(ih)] = dw
+                if ih == 0:
+                    dbs.append(db)
+        return dW, torch.cat(dbs)
+
+    rk1 = torch.zeros(3, W, **f32)
     rk1[0] = tape["w_sigma"]
-    # ---- feature layer: feat = Wf sin(f3 lin_c + phi3) + bf;  the rgb head feeds back through the same activation
-    s = sums()
-    dpre_c = abi.conv1x1_blocked_bwd(dfeat, tape["lin_c"], packT(g("feature_layer_linear.weight")), new(), s, mod=mods_d[3], act=1,
-                                     rk_w=rk3, rk_v=drgbp, **kw)
-    add_film(3, s)
-    dw, db = abi.act_wgrad_blocked(dfeat, tape["lin_c"], full, mods_d[3], act=1, **kw)
-    acc("feature_layer_linear.weight", dw)
-    acc("feature_layer_linear.bias", db)
-    del dfeat
-    # ---- colour layer: lin_c = Wcol' sin(f3 out3 + phi3) + bcol';  the sigma head feeds back through h4
-    f3 = mods_d[3][:, 0].contiguous()
-    s = sums()
+    # ---- feature layer: feat = Wf sin(f3 lin_c + phi3) + bf;  the rgb head feeds back through the same activation (rank 3)
+    dpre_c = dgrad(dfh, lin_c, _pad2(g("feature_layer_linear.weight").detach().float(), W, W), mods[3], film=3,
+                   rk_w=tape["w_rgb"], rk_v=drgbp)
+    dW, db = wgrad(dfh, lin_c, mods[3], None)
+    acc("feature_layer_linear.weight", dW[:Fd, :C])
+    acc("feature_layer_linear.bias", db[:Fd])
+    del dfh
+    # ---- colour layer: lin_c = Wcol' sin(f3 out3 + phi3) + bcol';  the sigma head feeds back through h4 (rank 1)
     wcol = g("color_layer_sine.layer.weight")
-    dpre = abi.conv1x1_blocked_bwd(dpre_c, outs[3], packT(wcol[:, 3:]), new(), s, mod=mods_d[3], act=1, ascale=f3,
-                                   rk_w=rk1, rk_v=dsig.reshape(B, 1, N), **kw)
-    add_film(3, s)
-    dw, db = abi.act_wgrad_blocked(dpre_c, outs[3], full, mods_d[3], act=1, pscale=f3, **kw)
+    dpre = dgrad(dpre_c, outs[3], _pad2(wcol[:, 3:].detach().float(), W, W), mods[3], film=3, ascale=scale(mods[3]),
+                 rk_w=rk1, rk_v=dsig.reshape(B, 1, N))
+    dW, db = wgrad(dpre_c, outs[3], mods[3], pscale(mods[3]))
     gw = torch.zeros_like(wcol)
-    gw[:, 3:] = dw
+    gw[:, 3:] = dW[:C, :C]
     acc("color_layer_sine.layer.weight", gw)
-    small = [(tape["bcol"], db)]                                              # bias + direction columns via autograd
+    small = [(tape["bcol"], db[:C])]                                          # bias + direction columns via autograd
     del dpre_c
     # ---- network.3 .. network.1: out_i = W_i sin(f_{i-1} out_{i-1} + phi_{i-1}) + b_i
     for i in (3, 2, 1):
-        fi = mods_d[i][:, 0].contiguous()
-        s = sums()
-        wi = g(f"network.{i}.layer.weight")
-        nxt = abi.conv1x1_blocked_bwd(dpre, outs[i - 1], packT(wi), new(), s, mod=mods_d[i - 1], act=1, ascale=fi, **kw)
-        add_film(i - 1, s)
-        dw, db = abi.act_wgrad_blocked(dpre, outs[i - 1], full, mods_d[i - 1], act=1, pscale=fi, **kw)
-        acc(f"network.{i}.layer.weight", dw)
-        acc(f"network.{i}.layer.bias", db)
+        wi = _pad2(g(f"network.{i}.layer.weight").detach().float(), W, W)
+        nxt = dgrad(dpre, outs[i - 1], wi, mods[i - 1], film=i - 1, ascale=scale(mods[i]))
+        dW, db = wgrad(dpre, outs[i - 1], mods[i - 1], pscale(mods[i]))
+        acc(f"network.{i}.layer.weight", dW[:C, :C])
+        acc(f"network.{i}.layer.bias", db[:C])
         dpre = nxt
-    # ---- network.0 (K = 512: coordinate half, geometry half) and the two first layers
-    f0 = mods_d[0][:, 0].contiguous()
-    w0 = g("network.0.layer.weight")
-    gw0 = torch.empty(H, 2 * H, **f32)
-    thirty = mod30[:, 0].contiguous()
-    for half, lin, first, cols in ((0, tape["lin_a"], "first_layer_coord.layer.", slice(0, 3)),
+    # ---- network.0 (K = 2C: coordinate part, geometry part) and the two first layers
+    w0 = g("network.0.layer.weight").detach().float()
+    gw0 = torch.empty(C, 2 * C, **f32)
+    for part, lin, first, cols in ((0, tape["lin_a"], "first_layer_coord.layer.", slice(0, 3)),
                                    (1, tape["lin_b"], "first_layer_mod.layer.", slice(3, 3 + tape["geo_dim"]))):
-        s = sums()
-        dlin = abi.conv1x1_blocked_bwd(dpre, lin, packT(w0[:, half * H:(half + 1) * H]), new(), s, mod=mod30, act=1, ascale=f0, **kw)
-        dw, db0 = abi.act_wgrad_blocked(dpre, lin, full, mod30, act=1, pscale=f0, **kw)
-        gw0[:, half * H:(half + 1) * H] = dw
+        dlin = dgrad(dpre, lin, _pad2(w0[:, part * C:(part + 1) * C], W, W), m30, ascale=scale(mods[0]))
+        dW, db0 = wgrad(dpre, lin, m30, pscale(mods[0]))
+        gw0[:, part * C:(part + 1) * C] = dW[:C, :C]
         # first layer: lin = W x + b with the sine's factor 30 folded into the incoming gradient
-        dwf, dbf = abi.act_wgrad_blocked(dlin, tape["rec_b"], T * 128 * 128, None, act=2, pscale=thirty, Cx=128, **kw)
-        acc(first + "weight", dwf[:, cols])
-        acc(first + "bias", dbf)
+        dwf, dbf = zip(*[abi.act_wgrad_blocked(dlin[h], tape["rec_b"], T * 128 * 128, None, act=2, pscale=m30[h][:, 0].contiguous(),
+                                               Cx=128, **kw) for h in halves])
+        acc(first + "weight", torch.cat(dwf)[:C, cols])
+        acc(first + "bias", torch.cat(dbf)[:C])
         del dlin
     acc("network.0.layer.weight", gw0)
-    acc("network.0.layer.bias", db0)
+    acc("network.0.layer.bias", db0[:C])
     # ---- FiLM tables, colour bias / direction columns: tiny autograd graphs
-    outs_, grads_ = list(tape["mods"]), list(dmods)
+    outs_ = [t for m in tape["mods_h"] for t in m]
+    grads_ = [t for m in dmods for t in m]
     for t, gr in small:
         if t.requires_grad:
             outs_.append(t)
@@ -252,7 +294,7 @@ class GeneratorCore(torch.autograd.Function):
             raise RuntimeError("hg3d: the training renderer is built for hierarchical_sample=False, lock_view_dependence=True")
         if cfg.get("neural_field_blocks", 4) != 4:
             raise RuntimeError("hg3d: the training renderer is built for neural_field_blocks == 4 (all shipped curricula)")
-        if cfg["hidden_dim"] != H:      # 384 / 420: the zero-padded forward of wide_ops with tapes, backward in wide_train
+        if cfg["hidden_dim"] != H:      # 384 / 420: the zero-padded forward of wide_ops, with tapes
             from . import wide_ops
             rtape, stape = {}, synthesis_train.SynthesisTape()
             feats, rgb01, depth = wide_ops.render_forward_wide(P, freq, phase, cond, cfg, u, noise, passes=passes, tape=rtape)
@@ -282,22 +324,10 @@ class GeneratorCore(torch.autograd.Function):
         B = stape.B
         Rh, Rw = cfg["render_height"], cfg["render_width"]
         grads = {}
-        if cfg["hidden_dim"] != H:
-            from . import wide_train
-            with torch.enable_grad():
-                dfs, dfeat = wide_train.synthesis_backward_wide(P, stape, d_rgb, passes=passes, grads=grads)
-                drgb = None if d_rgb_render is None else 2.0 * d_rgb_render.permute(0, 2, 3, 1).reshape(B, Rh * Rw, 3)
-                dfreq, dphase = wide_train.render_backward_wide(rtape, dfeat, drgb, grads=grads)
-        else:
-            with torch.enable_grad():
-                dfs, dfeat = synthesis_train.synthesis_backward(P, stape, d_rgb, passes=passes, grads=grads)
-            dray = torch.zeros(B, Rh * Rw, 260, dtype=torch.float32, device=d_rgb.device)
-            if dfeat is not None:
-                dray[..., :256] = dfeat
-            if d_rgb_render is not None:
-                dray[..., 256:259] = 2.0 * d_rgb_render.permute(0, 2, 3, 1).reshape(B, Rh * Rw, 3)
-            with torch.enable_grad():
-                dfreq, dphase = mlp_backward(rtape, dray, grads=grads)
+        with torch.enable_grad():
+            dfs, dfeat = synthesis_train.synthesis_backward(P, stape, d_rgb, passes=passes, grads=grads)
+            drgb = None if d_rgb_render is None else 2.0 * d_rgb_render.permute(0, 2, 3, 1).reshape(B, Rh * Rw, 3)
+            dfreq, dphase = mlp_backward(rtape, dfeat, drgb, grads=grads)
         ctx.tapes = None
         # Every returned gradient must own its storage: autograd's AccumulateGrad steals a returned tensor as `.grad` when
         # nobody else holds the TensorImpl, so two parameters whose gradients are views of one buffer (the nine ToRGB biases

@@ -5,12 +5,14 @@ input is kept (18 activations of B*HW*256 fp32 -- 2.1 GB each at the C2 workload
 and every [B,C]- / [C]-sized quantity the kernels consume (folded BatchNorm+SPADE tables, spectrally
 normalised weights) is built with torch autograd from its leaves.
 
-Backward (autograd through SynthesisNetwork.forward map3d_generator.py:58-97, SPADEBlock.forward
-map3d_layers.py:218-238, SPADE2d.forward :176-190, ToRGB :346-352, SynthesisInput :260-275), walking the
-half-blocks in reverse; per half-block
-    hg_spade_bwd_combine  dL/dout   from the next half-block's dpre (+ skip gradient, + ToRGB^T drgb)
-    hg_spade_bwd_dgrad    dpre = (W^T dL/dout) * lrelu'(pre), S1 = sum dpre, S2 = sum dpre*x     (wgmma)
-    hg_spade_bwd_wgrad    dW = dL/dout . y^T, dbias                                              (wgmma)
+Backward (`synthesis_backward`, one for every width: autograd through SynthesisNetwork.forward
+map3d_generator.py:58-97, SPADEBlock.forward map3d_layers.py:218-238, SPADE2d.forward :176-190, ToRGB :346-352,
+SynthesisInput :260-275), walking the half-blocks in reverse over the tape's 256-channel halves (one here, two from
+the zero-padded forward of modules/wide_ops.py at hidden_dim 384 / 420; see `SynthesisTape`); per half-block
+    hg_spade_bwd_combine  dL/dout   from the next half-block's dpre (+ skip gradient, + ToRGB^T drgb)   per half
+    hg_spade_bwd_dgrad    dpre = (W^T dL/dout) * lrelu'(pre), S1 = sum dpre, S2 = sum dpre*x     (wgmma; with two
+                          halves hg_conv1x1_blocked_bwd per input half, K = 512)
+    hg_spade_bwd_wgrad    dW = dL/dout . y^T, dbias                    (wgmma; per (output half, input half) block)
 and the small chains on the host side: d(g1,g0) = (S2,S1) -> BatchNorm weight/bias, gamma/beta MLP, fixed style,
 and -- through the leaves sum(x), sum(x^2) of the batch statistics -- the a[c] + k[c]*x term of dL/dx
 (SyncBatchNorm: those two leaf gradients are SUM-all-reduced, like the statistics themselves).
@@ -22,10 +24,10 @@ keep the fused forward kernel and, in backward, REBUILD their per-pixel quantiti
     hg_spade_pixel_pre     pre = (x*sc + sh)*gam + bet
 then the same dgrad / wgrad kernels run on `pre`, followed by
     hg_spade_pixel_mod_bwd dxn = dpre*gam, dgam = dpre*xn (+ the BatchNorm / bias sums)
-    hg_conv1x1_blocked_bwd dA1 = ([dgam | dpre] . [Wg | Wb]) * relu'(A1)        (wgmma, K = 512, pixel-major out)
+    hg_conv1x1_blocked_bwd dA1 = ([dgam | dpre] . [Wg | Wb]) * relu'(A1)        (wgmma, K = 512 launches, pixel-major out)
     hg_wgrad_blocked   x2  dWg = dgam . A1^T,  dWb = dpre . A1^T                 (wgmma)
     hg_bilinear_adjoint    dP_lr (render resolution)
-and once, at the end, d(feature maps) = dP_lr . W_shared (wgmma `hg_linear`) and dW_shared = dP_lr^T . features
+and once, at the end, d(feature maps) = dP_lr . W_shared (wgmma `hg_linear`, K <= 256 per launch) and dW_shared = dP_lr^T . features
 (a plain library GEMM through torch.matmul).
 """
 from __future__ import annotations
@@ -35,16 +37,32 @@ import torch.distributed as dist
 import torch.nn.functional as F
 
 from .. import abi
+from ..ops.dense import _gemm_nt
 from .synthesis_ops import STAT_STRIDE, _PtrView, _gamma_beta_interleaved, _spade, all_reduce_stats, is_pixel_style, sn_weights
+from .wide_ops import HALF, _pad2
 
 C = 256
 
 
 class SynthesisTape:
-    """Everything `synthesis_backward` needs from one training forward."""
+    """Everything `synthesis_backward` needs from one training forward: `synthesis_forward_train` at hidden_dim 256,
+    `wide_ops.synthesis_forward_wide(..., tape=tape)` at the zero-padded widths.
+
+    Every activation is a tuple of nh tile-blocked 256-channel halves [B,T,256,128], nh = 1 at 256 and 2 at the padded
+    widths (padded channels hold zeros).  `halves` has one record per half-block:
+        x, out          per-half tuples of its input and output
+        x_bstride       the batch stride of x: 0 for the batch-shared synthesis input [T,256,128] at 256, T*256*128 otherwise
+        mod_d           per-half tuple of the detached folded table: [B,2,256] const style, (sc, sh) [2,256] pixel style
+        mod, ssum, ssq  the same table over nh*256 channels, with autograd history from the batch-statistics leaves
+                        ssum = sum(x), ssq = sum(x^2)
+        w_sn            W / sigma with history; conv, the convolution's parameter prefix
+        rgb, rgb_w      the ToRGB parameter prefix and its weight [3,nh*256] (None without ToRGB); skip_from
+        pixel           pixel style; then also i (its slice of P_lr), spade, p_bias (with history), p_bias_d and
+                        wg, wb [nh*256,128], bg1 = gamma bias + 1, bb [nh*256]
+    `input` holds the synthesis input's w [nh*256,2], b [nh*256], ic, jc and parameter prefix."""
 
     def __init__(self):
-        self.halves = []      # per half-block: dict(x, x_bstride, mod, w_sn, ssum, ssq, conv, skip_from, rgb_w ...)
+        self.halves = []
         self.cfg = None
         self.B = 0
         self.rgb = None
@@ -110,7 +128,7 @@ def synthesis_forward_train(params, feat_lr, fixed_style, cfg, *, passes=3, pref
     x0 = torch.empty(T, C, 128, **f32)
     w_in = P[input_prefix + "network.0.weight"].detach().reshape(C, 2).contiguous()
     abi.synth_input(w_in, P[input_prefix + "network.0.bias"].detach(), ic, jc, x0, stats[0], B)
-    tape.input = dict(w=w_in, ic=ic, jc=jc, prefix=input_prefix)
+    tape.input = dict(w=w_in, b=P[input_prefix + "network.0.bias"].detach(), ic=ic, jc=jc, prefix=input_prefix)
 
     # spectral normalisation of the 18 convolutions: one launch (power iteration, buffers in place), W / sigma with history
     w_sns = sn_weights(P, [blk(k) + f"conv_{j}." for k, j in halves], True)
@@ -146,8 +164,8 @@ def synthesis_forward_train(params, feat_lr, fixed_style, cfg, *, passes=3, pref
             kw = dict(rgb_w=P[rgb_name + "weight"].detach().reshape(3, C).contiguous(), rgb_b=P[rgb_name + "bias"].detach(),
                       rgb_in=rgb_cur, rgb_out=rgb_next)
         mod_d = mod.detach().contiguous()
-        rec = dict(x=cur, x_bstride=cur_bstride, mod=mod, mod_d=mod_d, w_sn=w_sn, ssum=ssum, ssq=ssq, conv=conv,
-                   skip_from=block_in[2] if use_skip else None, rgb=rgb_name, out=out, pixel=pixel)
+        rec = dict(x=(cur,), x_bstride=cur_bstride, mod=mod, mod_d=(mod_d,), w_sn=w_sn, ssum=ssum, ssq=ssq, conv=conv,
+                   skip_from=block_in[2] if use_skip else None, rgb=rgb_name, rgb_w=kw.get("rgb_w"), out=(out,), pixel=pixel)
         if pixel:
             i = pxi[(k, j)]
             s_ = sp(k, j)
@@ -218,53 +236,79 @@ def grad_accumulator(P, grads):
     return acc
 
 
+def _packT(W, ih):
+    """Operand image of the transposed input-half `ih` columns of a zero-padded [nh*256, nh*256] weight: the data
+    gradient's [256 x K = nh*256] weight."""
+    return abi.pack_weight(W[:, ih * HALF:(ih + 1) * HALF].t().contiguous(), Nb=256)[0]
+
+
 def synthesis_backward(params, tape, drgb, *, passes=3, grads=None):
-    """Gradients of every synthesis parameter in `params` (those that require grad) into `grads` (name -> tensor; `.grad`
-    when grads is None) and returns (d fixed_style [B,256], d feat_lr [B,Rh*Rw,256] or None when no half-block is
-    pixel-style)."""
+    """Backward of the training synthesis network at every width (the tape format is `SynthesisTape`'s): gradients of
+    every synthesis parameter in `params` that requires grad into `grads` (name -> tensor; `.grad` when grads is None);
+    returns (d fixed_style [B,C], d feat_lr [B,Rh*Rw,C] or None when no half-block is pixel-style).  A layer over nh
+    halves is a data-gradient launch per input half (K = nh*256 from the output halves' gradients) and a weight-gradient
+    launch per (output half, input half) block; padded channels carry zero weights and tables, so their gradients are
+    zero up to the trimming to each parameter's shape."""
     P = params
     cfg, B = tape.cfg, tape.B
+    C = cfg["hidden_dim"]
     Hg, Wg = cfg["gen_height"], cfg["gen_width"]
     HW = Hg * Wg
     T = (HW + 127) // 128
     dev = drgb.device
     f32 = dict(dtype=torch.float32, device=dev)
+    kw = dict(B=B, Hg=Hg, Wg=Wg, passes=passes)
     drgb = drgb.reshape(B, 3, HW).float().contiguous()
     H = tape.halves
     n = len(H)
-    full = T * C * 128
-
+    nh = len(H[0]["x"])
+    halves = range(nh)
+    W2 = nh * HALF
+    sl = lambda c: slice(c * HALF, (c + 1) * HALF)
+    full = T * HALF * 128
+    new = lambda: torch.empty(B, T, HALF, 128, **f32)
     acc = grad_accumulator(P, grads)
+
+    def conv_wgrad(d, xs, x_bstride, mods_in):
+        """[nh*256, nh*256] weight gradient of a half-block's convolution block by block, [nh*256] bias gradient."""
+        dW = torch.empty(W2, W2, **f32)
+        dbs = []
+        for oh in halves:
+            for ih in halves:
+                dw, db = abi.spade_bwd_wgrad(d[oh], xs[ih], x_bstride, mods_in[ih], want_bias=ih == 0, **kw)
+                dW[sl(oh), sl(ih)] = dw
+                if ih == 0:
+                    dbs.append(db)
+        return dW, torch.cat(dbs)
 
     # every ToRGB bias sees the full drgb
     drgb_sum = drgb.sum((0, 2))
-    small_out, small_grad = [], []          # (tensor with autograd history, its gradient): one autograd.backward at the end
-    dout = {}                               # half index -> dL/d(out of that half)   (only the live ones are kept)
-    nxt = None                              # (dpre, g1 table [B,2,C], ak [2,C]) of half h+1
+    small_out, small_grad = [], []          # (tensor with autograd history, its gradient): one autograd pass at the end
+    dout = {}                               # half-block index -> dL/d(its out) per half   (only the live ones are kept)
+    nxt = None                              # (dpre, g1 table, ak) per half of half-block h+1
     for h in range(n - 1, -1, -1):
         rec = H[h]
-        # ---- dL/d(out_h): from half h+1 (dpre*g1 + a + k*x), the skip of the block two halves later, ToRGB
-        dskip = None
+        # ---- dL/d(out_h): from half-block h+1 (dpre*g1 + a + k*x), the skip of the block two half-blocks later, ToRGB
+        dskip = (None,) * nh
         if h + 2 < n and H[h + 2]["skip_from"] == h + 1:      # out_h is the input of a block with a residual skip
             dskip = dout[h + 2]
-        d = torch.empty(B, T, C, 128, **f32)
-        dwrgb = None
-        kw = {}
+        d, dwrgb = [], []
+        for c in halves:
+            ckw = {}
+            if rec["rgb"] is not None:
+                dwrgb.append(torch.zeros(3, HALF, dtype=torch.float64, device=dev))
+                ckw = dict(drgb=drgb, rgb_w=rec["rgb_w"][:, sl(c)].contiguous(), dwrgb=dwrgb[c])
+            if nxt is not None:
+                ckw.update(dpre=nxt[0][c], g1=nxt[1][c], ak=nxt[2][c])
+            d.append(abi.spade_bwd_combine(new(), B=B, Hg=Hg, Wg=Wg, x=rec["out"][c], x_bstride=full, dskip=dskip[c], **ckw))
         if rec["rgb"] is not None:
-            dwrgb = torch.zeros(3, C, dtype=torch.float64, device=dev)
-            kw = dict(drgb=drgb, rgb_w=P[rec["rgb"] + "weight"].detach().reshape(3, C).contiguous(), dwrgb=dwrgb)
-        if nxt is not None:
-            kw.update(dpre=nxt[0], g1=nxt[1], ak=nxt[2])
-        abi.spade_bwd_combine(d, B=B, Hg=Hg, Wg=Wg, x=rec["out"], x_bstride=full, dskip=dskip, **kw)
-        if dwrgb is not None:
-            acc(rec["rgb"] + "weight", dwrgb.float())
+            acc(rec["rgb"] + "weight", torch.cat(dwrgb, -1)[:, :C].float())
             acc(rec["rgb"] + "bias", drgb_sum)
         dout[h] = d
         dout.pop(h + 3, None)
-        # ---- this half-block
-        wimg_t = abi.pack_weight(rec["w_sn"].detach().t().contiguous(), Nb=256)[0]
-        dpre = torch.empty(B, T, C, 128, **f32)
-        sums = torch.zeros(B, 2, C, dtype=torch.float64, device=dev)
+        # ---- this half-block: const style acts on x through its table, pixel style on the rebuilt `pre`
+        Wsn = _pad2(rec["w_sn"].detach().reshape(C, C), W2, W2)
+        sums = [torch.zeros(B, 2, HALF, dtype=torch.float64, device=dev) for _ in halves]
         if rec["pixel"]:
             Rh, Rw = cfg["render_height"], cfg["render_width"]
             i = rec["i"]
@@ -272,36 +316,41 @@ def synthesis_backward(params, tape, drgb, *, passes=3, grads=None):
             # rebuild A1, gamma, beta, pre
             a1 = torch.empty(B, T, 128, 128, **f32)
             abi.spade_a1(_PtrView(p_lr[:, i * 128:]), p_lr.shape[1], rec["p_bias_d"], a1, B=B, Hg=Hg, Wg=Wg, Rh=Rh, Rw=Rw)
-            gam = torch.empty(B, T, C, 128, **f32)
-            pre = torch.empty(B, T, C, 128, **f32)
-            abi.conv1x1_blocked(a1, 128, abi.pack_weight(rec["wg"].contiguous(), Nb=256)[0], rec["bg1"], gam, B=B, Hg=Hg, Wg=Wg, passes=passes)
-            abi.conv1x1_blocked(a1, 128, abi.pack_weight(rec["wb"].contiguous(), Nb=256)[0], rec["bb"], pre, B=B, Hg=Hg, Wg=Wg, passes=passes)
-            abi.spade_pixel_pre(rec["x"], rec["x_bstride"], rec["mod_d"], gam, pre, B=B, Hg=Hg, Wg=Wg)
-            if getattr(tape, "keep_masks", False):      # tests: the LeakyReLU mask this backward differentiates through
-                rec["mask"] = pre > 0
+            gam, pre = [], []
+            for c in halves:
+                gam.append(abi.conv1x1_blocked(a1, 128, abi.pack_weight(rec["wg"][sl(c)].contiguous(), Nb=256)[0],
+                                               rec["bg1"][sl(c)].contiguous(), new(), **kw))
+                pre.append(abi.conv1x1_blocked(a1, 128, abi.pack_weight(rec["wb"][sl(c)].contiguous(), Nb=256)[0],
+                                               rec["bb"][sl(c)].contiguous(), new(), **kw))
+                abi.spade_pixel_pre(rec["x"][c], rec["x_bstride"], rec["mod_d"][c], gam[c], pre[c], B=B, Hg=Hg, Wg=Wg)
+            if getattr(tape, "keep_masks", False):      # tests: the masks this backward differentiates through
+                rec["mask"] = [p > 0 for p in pre]
                 rec["mask_a1"] = a1 > 0
             # conv data / weight gradients on pre (y = lrelu(pre))
-            abi.conv1x1_blocked_bwd(d, pre, wimg_t, dpre, sums, B=B, Hg=Hg, Wg=Wg, passes=passes)
-            dw, db = abi.spade_bwd_wgrad(d, pre, full, None, B=B, Hg=Hg, Wg=Wg, passes=passes)
+            dpre = [abi.conv1x1_blocked_bwd(d[0], pre[c], _packT(Wsn, c), new(), sums[c], g2=d[1] if nh == 2 else None, **kw)
+                    for c in halves]
+            dW, db = conv_wgrad(d, pre, full, (None,) * nh)
             # modulation: dxn (over pre), dgam (over gam), BatchNorm scale/shift sums
-            s3 = torch.zeros(3, C, dtype=torch.float64, device=dev)
-            abi.spade_pixel_mod_bwd(dpre, rec["x"], rec["x_bstride"], rec["mod_d"], gam, pre, s3, B=B, Hg=Hg, Wg=Wg)
+            s3 = [torch.zeros(3, HALF, dtype=torch.float64, device=dev) for _ in halves]
+            for c in halves:
+                abi.spade_pixel_mod_bwd(dpre[c], rec["x"][c], rec["x_bstride"], rec["mod_d"][c], gam[c], pre[c], s3[c], B=B, Hg=Hg, Wg=Wg)
             dxn, dgam = pre, gam
-            # gamma/beta MLP: hidden-layer gradient (ReLU mask from A1), weight gradients, bilinear adjoint
-            w7 = torch.zeros(256, 512, **f32)
-            w7[:128, :256] = rec["wg"].t()
-            w7[:128, 256:] = rec["wb"].t()
-            da1 = torch.empty(B, HW, 128, **f32)
+            # gamma/beta MLP: dA1 = ([dgam halves, dpre halves] . [Wg | Wb]) * relu'(A1), K = 2*nh*256 in K = 512 launches
+            srcs = dgam + dpre
+            wt = torch.cat([rec["wg"], rec["wb"]]).t()                        # [128, 2*nh*256]
             s7 = torch.zeros(B, 2, 128, dtype=torch.float64, device=dev)
-            abi.conv1x1_blocked_bwd(dgam, a1, abi.pack_weight(w7, Nb=256)[0], da1, s7, g2=dpre, Cout=128, slope=0.0,
-                                    pixel_major=True, B=B, Hg=Hg, Wg=Wg, passes=passes)
-            dwg, dbg = abi.spade_bwd_wgrad(dgam, a1, T * 128 * 128, None, Cx=128, B=B, Hg=Hg, Wg=Wg, passes=passes)
-            dwb, dbb = abi.spade_bwd_wgrad(dpre, a1, T * 128 * 128, None, Cx=128, B=B, Hg=Hg, Wg=Wg, passes=passes)
+            da1 = None
+            for k in range(0, len(srcs), 2):
+                w7 = torch.zeros(256, 2 * HALF, **f32)
+                w7[:128] = wt[:, k * HALF:(k + 2) * HALF]
+                part = abi.conv1x1_blocked_bwd(srcs[k], a1, abi.pack_weight(w7, Nb=256)[0], torch.empty(B, HW, 128, **f32), s7,
+                                               g2=srcs[k + 1], Cout=128, slope=0.0, pixel_major=True, **kw)
+                da1 = part if da1 is None else da1.add_(part)
             sp_ = rec["spade"]
-            acc(sp_ + "mlp_gamma.weight", dwg)
-            acc(sp_ + "mlp_gamma.bias", dbg)
-            acc(sp_ + "mlp_beta.weight", dwb)
-            acc(sp_ + "mlp_beta.bias", dbb)
+            for gs, nm in ((dgam, "mlp_gamma."), (dpre, "mlp_beta.")):
+                dws, dbs = zip(*[abi.spade_bwd_wgrad(gs[c], a1, T * 128 * 128, None, Cx=128, **kw) for c in halves])
+                acc(sp_ + nm + "weight", torch.cat(dws)[:C])
+                acc(sp_ + nm + "bias", torch.cat(dbs)[:C])
             if "dp" not in tape.p:
                 tape.p["dp"] = torch.zeros_like(p_lr)
             dp = tape.p["dp"]
@@ -309,60 +358,62 @@ def synthesis_backward(params, tape, drgb, *, passes=3, grads=None):
             if rec["p_bias"].requires_grad:
                 small_out.append(rec["p_bias"])
                 small_grad.append(s7[:, 0].float())
-            acc(rec["conv"] + "bias", db)
-            small_out.append(rec["w_sn"])
-            small_grad.append(dw)
-            dmod = torch.stack([s3[0], s3[1]]).float()                        # d sc = sum dxn*x, d sh = sum dxn
+            # d sc = sum dxn*x, d sh = sum dxn
+            dmod = torch.stack([torch.cat([s[0] for s in s3]), torch.cat([s[1] for s in s3])]).float()
             dpre = dxn
-            g1_tab = rec["mod_d"][0][None, None, :].expand(B, 2, C).contiguous()
-            del a1, da1
+            g1_tab = [m[0][None, None, :].expand(B, 2, HALF).contiguous() for m in rec["mod_d"]]
+            del a1, da1, gam
         else:
-            abi.spade_bwd_dgrad(d, rec["x"], rec["x_bstride"], rec["mod_d"], wimg_t, dpre, sums, B=B, Hg=Hg, Wg=Wg, passes=passes)
-            dw, db = abi.spade_bwd_wgrad(d, rec["x"], rec["x_bstride"], rec["mod_d"], B=B, Hg=Hg, Wg=Wg, passes=passes)
-            acc(rec["conv"] + "bias", db)
-            small_out.append(rec["w_sn"])
-            small_grad.append(dw)
-            dmod = torch.stack([sums[:, 1], sums[:, 0]], dim=1).float()       # d g1 = sum dpre*x, d g0 = sum dpre
+            if nh == 1:     # the only data-gradient entry point that reads a batch-shared input (block 0 at 256)
+                dpre = [abi.spade_bwd_dgrad(d[0], rec["x"][0], rec["x_bstride"], rec["mod_d"][0], _packT(Wsn, 0), new(), sums[0], **kw)]
+            else:
+                dpre = [abi.conv1x1_blocked_bwd(d[0], rec["x"][c], _packT(Wsn, c), new(), sums[c], g2=d[1], mod=rec["mod_d"][c],
+                                                slope=0.2, **kw) for c in halves]
+            dW, db = conv_wgrad(d, rec["x"], rec["x_bstride"], rec["mod_d"])
+            # d g1 = sum dpre*x, d g0 = sum dpre
+            dmod = torch.stack([torch.cat([s[:, 1] for s in sums], -1), torch.cat([s[:, 0] for s in sums], -1)], dim=1).float()
             g1_tab = rec["mod_d"]
+        acc(rec["conv"] + "bias", db[:C])
+        small_out.append(rec["w_sn"])
+        small_grad.append(dW[:C, :C].reshape(rec["w_sn"].shape))
         ga, gk = torch.autograd.grad(rec["mod"], [rec["ssum"], rec["ssq"]], grad_outputs=dmod, retain_graph=True)
         ak = torch.stack([ga, gk])
-        if tape.world > 1:          # every rank's loss depends on the global statistics
+        if tape.world > 1:          # SyncBatchNorm: every rank's loss depends on the global statistics
             dist.all_reduce(ak, group=tape.process_group)
-        ak = torch.stack([ak[0], 2.0 * ak[1]]).float().contiguous()      # d(sum x)/dx = 1, d(sum x^2)/dx = 2x
+        ak = torch.stack([ak[0], 2.0 * ak[1]]).float()                     # d(sum x)/dx = 1, d(sum x^2)/dx = 2x
         small_out.append(rec["mod"])
         small_grad.append(dmod)
-        nxt = (dpre, g1_tab, ak)
-    # ---- gradient w.r.t. the shared synthesis input x0, then its two parameters
-    dx0 = torch.empty(B, T, C, 128, **f32)
-    abi.spade_bwd_combine(dx0, B=B, Hg=Hg, Wg=Wg, x=H[0]["x"], x_bstride=0, dpre=nxt[0], g1=nxt[1], ak=nxt[2])
+        nxt = (dpre, g1_tab, [ak[:, sl(c)].contiguous() for c in halves])
+    # ---- gradient w.r.t. the synthesis input, then its two parameters, per half
     ip = tape.input["prefix"]
-    dw_in, db_in = abi.synth_input_bwd(dx0, tape.input["w"], P[ip + "network.0.bias"].detach(), tape.input["ic"], tape.input["jc"], B)
-    acc(ip + "network.0.weight", dw_in)
-    acc(ip + "network.0.bias", db_in)
-    # ---- all [C]- and [B,C]-sized chains in one autograd pass (accumulates into the Parameters' .grad)
+    dw_in, db_in = [], []
+    for c in halves:
+        dx0 = abi.spade_bwd_combine(new(), B=B, Hg=Hg, Wg=Wg, x=H[0]["x"][c], x_bstride=H[0]["x_bstride"], dpre=nxt[0][c], g1=nxt[1][c],
+                                    ak=nxt[2][c])
+        dw, db = abi.synth_input_bwd(dx0, tape.input["w"][sl(c)].contiguous(), tape.input["b"][sl(c)].contiguous(),
+                                     tape.input["ic"], tape.input["jc"], B)
+        dw_in.append(dw)
+        db_in.append(db)
+    acc(ip + "network.0.weight", torch.cat(dw_in)[:C])
+    acc(ip + "network.0.bias", torch.cat(db_in)[:C])
+    # ---- all [C]- and [B,C]-sized chains in one autograd pass
     fs = tape.fixed_style
     leaves = [t for t in small_out if t.requires_grad]
     small = [g for t, g in zip(small_out, small_grad) if t.requires_grad]
-    names = [n for n, p in P.items() if isinstance(p, torch.Tensor) and p.requires_grad and p.is_leaf]
-    res = torch.autograd.grad(leaves, [P[n] for n in names] + [fs], small, allow_unused=True)
-    for n, r in zip(names, res[:-1]):
+    names = [k for k, p in P.items() if isinstance(p, torch.Tensor) and p.requires_grad and p.is_leaf]
+    res = torch.autograd.grad(leaves, [P[k] for k in names] + [fs], small, allow_unused=True)
+    for k, r in zip(names, res[:-1]):
         if r is not None:
-            acc(n, r)
+            acc(k, r)
     dfs = res[-1] if res[-1] is not None else torch.zeros_like(fs)
     # ---- render-resolution projection P_lr = X . W_shared^T: feature-map and weight gradients
     dfeat = None
     if tape.px and "dp" in tape.p:
         dp, Ws, X = tape.p["dp"], tape.p["Ws"], tape.p["X"]
-        WsT = Ws.t().contiguous()                                                    # [256, n*128]
-        dfeat = None
-        for c0 in range(0, WsT.shape[1], 256):        # hg_linear takes K <= 256: one product per pair of half-blocks
-            img, Nb = abi.pack_weight(WsT[:, c0:c0 + 256].contiguous(), Nb=256)
-            part = abi.linear(dp[:, c0:c0 + 256], img, Nb, C, passes=passes)
-            dfeat = part if dfeat is None else dfeat.add_(part)
-        dfeat = dfeat.reshape(B, -1, C)
+        dfeat = _gemm_nt(dp, Ws.t().contiguous(), passes=passes).reshape(B, -1, C)
         prev = torch.backends.cuda.matmul.allow_tf32
         torch.backends.cuda.matmul.allow_tf32 = False
-        dWs = dp.t() @ X                                                             # [n*128, 256]  (plain library GEMM)
+        dWs = dp.t() @ X                                                             # [n*128, C]  (plain library GEMM)
         torch.backends.cuda.matmul.allow_tf32 = prev
         for rec in H:
             if rec["pixel"]:

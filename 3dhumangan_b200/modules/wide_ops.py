@@ -16,7 +16,8 @@ affine and zero FiLM tables, so they stay zero through every layer.
              an identity table -- the decomposition the 256-channel BACKWARD already uses.
 
 Inference and train-mode forward (batch statistics, running-stat and spectral-norm buffer updates).  Given a `tape`,
-each forward also keeps what its backward (modules/wide_train.py) needs, and builds the small tables that carry
+each forward also keeps what the backward of every width needs (render_train.mlp_backward,
+synthesis_train.synthesis_backward, over two 256-channel halves here), and builds the small tables that carry
 parameter gradients (FiLM, SPADE / BatchNorm, W / sigma) with autograd history.  Mirrors Map3DGenerator.render / forward (map3d_generator.py:208-280, 381-523),
 COORDCONCATSIREN.forward (modulated.py:41-75), SynthesisNetwork.forward (map3d_generator.py:58-97).
 """
@@ -83,8 +84,9 @@ def wide_layer(xs, W512, b512, *, mods=None, act=0, slope=0.2, skips=None, stats
 @torch.no_grad()
 def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix="neural_field.", tape=None):
     """-> ray features [B,R,C], rgb [B,R,3] (in [0,1], before the *2-1), depth [B,R,1].
-    `tape` (a dict) receives what `wide_train.render_backward_wide` needs: per half the linear outputs lin_a, lin_b,
-    out_0..3, lin_c, feat, then sig, rgbp and the FiLM tables built from freq / phase leaves with autograd history."""
+    `tape` (a dict) receives what `render_train.mlp_backward` needs, in the format its docstring describes: per half the
+    linear outputs lin_a, lin_b, out_0..3, lin_c, feat, then sig, rgbp and the FiLM tables built from freq / phase
+    leaves with autograd history."""
     from . import render_train
     abi.require_device()
     g = lambda n: P[prefix + n].detach().float()
@@ -191,9 +193,9 @@ def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix
 def synthesis_forward_wide(P, feats, fixed_style, cfg, *, training=True, passes=3, prefix="synthesis_network.",
                            input_prefix="synthesis_input.", process_group=None, tape=None):
     """feats [B, Rh*Rw, C] render-resolution features, fixed_style [B,C] -> rgb [B,3,Hg,Wg].
-    `tape` (a `synthesis_train.SynthesisTape`, training only) receives what `wide_train.synthesis_backward_wide` needs: per
-    half-block its input halves, the SPADE tables built with autograd from sum(x) / sum(x^2) leaves (instead of
-    hg_bn_finalize), W / sigma with history and the skip / ToRGB bookkeeping, as `synthesis_train` keeps them."""
+    `tape` (a `synthesis_train.SynthesisTape`, training only) receives what `synthesis_train.synthesis_backward` needs:
+    per half-block its input halves, the SPADE tables built with autograd from sum(x) / sum(x^2) leaves (instead of
+    hg_bn_finalize), W / sigma with history and the skip / ToRGB bookkeeping, in the format of that class."""
     abi.require_device()
     dev = feats.device
     B = feats.shape[0]
@@ -295,8 +297,8 @@ def synthesis_forward_wide(P, feats, fixed_style, cfg, *, training=True, passes=
                        out0=torch.empty(B, 3, HW, **f32), out1=torch.empty(B, 3, HW, **f32))
         srows = (stats[idx + 1, 0], stats[idx + 1, 1]) if training else None
         if taped:
-            rec = dict(x=cur, mod=mod, mod_d=tables, w_sn=w_sns[conv], ssum=ssum, ssq=ssq, conv=conv, pixel=pixel,
-                       skip_from=block_in[1] if use_skip else None, rgb=name, rgb_w=None if rgb is None else rgb["w"])
+            rec = dict(x=cur, x_bstride=full, mod=mod, mod_d=tuple(tables), w_sn=w_sns[conv], ssum=ssum, ssq=ssq, conv=conv,
+                       pixel=pixel, skip_from=block_in[1] if use_skip else None, rgb=name, rgb_w=None if rgb is None else rgb["w"])
             tape.halves.append(rec)
         if pixel:
             i = pxi[(k, j)]

@@ -134,8 +134,9 @@ def test_combine(with_rgb, with_skip, with_dpre):
         assert (dwrgb.cpu() - dw_ref).abs().max() / dw_ref.abs().max() < 1e-5
 
 
-def _network_case(port, monkeypatch, mod_blocks, mode, Rh, Rw, seed):
-    """Whole-network gradients against fp64 autograd through the restated reference on the CPU.
+def _network_case(port, monkeypatch, mod_blocks, mode, Rh, Rw, seed, C=C):
+    """Whole-network gradients against fp64 autograd through the restated reference on the CPU, at hidden_dim 256
+    (synthesis_train's forward) or a zero-padded width (wide_ops' forward); one backward serves both.
 
     The gradient is DISCONTINUOUS in the LeakyReLU masks: a pre-activation that rounds to the other side of zero
     changes its contribution by a factor 5, so even torch-fp32 vs torch-fp64 gradients of this network differ by
@@ -145,8 +146,10 @@ def _network_case(port, monkeypatch, mod_blocks, mode, Rh, Rw, seed):
     import torch.nn.functional as TF
     pkg = importlib.import_module("3dhumangan_b200")
     st = importlib.import_module("3dhumangan_b200.modules.synthesis_train")
+    wo = importlib.import_module("3dhumangan_b200.modules.wide_ops")
     cfg = pkg.configs.baseline_config("tiny")
-    cfg.update(gen_height=16, gen_width=24, render_height=Rh, render_width=Rw, mod_blocks=mod_blocks, map3d_mode=mode)
+    cfg.update(hidden_dim=C, feature_dim=C, gen_height=16, gen_width=24, render_height=Rh, render_width=Rw, mod_blocks=mod_blocks,
+               map3d_mode=mode)
     B, Hg, Wg = 2, cfg["gen_height"], cfg["gen_width"]
     HW = Hg * Wg
     params = port.init_generator_params(cfg, seed=seed)
@@ -162,22 +165,28 @@ def _network_case(port, monkeypatch, mod_blocks, mode, Rh, Rw, seed):
     for n in learn:
         pg[n].requires_grad_(True)
     feat_lr = fmap.permute(0, 2, 3, 1).reshape(B, Rh * Rw, C).contiguous().cuda()
-    rgb, tape = st.synthesis_forward_train(pg, feat_lr, fixed.cuda(), cfg)
+    if C == 256:
+        rgb, tape = st.synthesis_forward_train(pg, feat_lr, fixed.cuda(), cfg)
+    else:
+        tape = st.SynthesisTape()
+        rgb = wo.synthesis_forward_wide(pg, feat_lr, fixed.cuda(), cfg, training=True, tape=tape)
     tape.keep_masks = True
     dfs, dfeat = st.synthesis_backward(pg, tape, wgt.cuda())
     torch.cuda.synchronize()
+
+    def planar(halves):
+        """Per-half tile-blocked activations (batch-shared ones expanded) -> [B,C,HW] without the padded channels."""
+        return torch.cat([_planar(t.expand(B, -1, -1, -1), HW) for t in halves], 1)[:, :C].cpu()
+
     masks, relu_masks = [], []
     for rec in tape.halves:
         if rec["pixel"]:
-            mk = rec["mask"].permute(0, 2, 1, 3).reshape(B, C, -1)[:, :, :HW].cpu()
-            masks.append(torch.where(mk, 1.0, 0.2).double().reshape(B, C, Hg, Wg))
-            ma = rec["mask_a1"].permute(0, 2, 1, 3).reshape(B, 128, -1)[:, :, :HW].cpu()
-            relu_masks.append(ma.double().reshape(B, 128, Hg, Wg))     # ReLU of the gamma/beta hidden layer
+            masks.append(torch.where(planar(rec["mask"]), 1.0, 0.2).double().reshape(B, C, Hg, Wg))
+            relu_masks.append(_planar(rec["mask_a1"], HW).cpu().double().reshape(B, 128, Hg, Wg))     # ReLU of the gamma/beta MLP
             continue
         relu_masks.append(None)
-        x = rec["x"] if rec["x"].dim() == 4 else rec["x"][None].expand(B, -1, -1, -1)
-        xp = x.permute(0, 2, 1, 3).reshape(B, C, -1)[:, :, :HW].double().cpu()
-        m = rec["mod_d"].double().cpu()
+        xp = planar(rec["x"]).double()
+        m = torch.cat(rec["mod_d"], -1)[..., :C].double().cpu()
         pre = xp * m[:, 0, :, None] + m[:, 1, :, None]
         masks.append(torch.where(pre > 0, 1.0, 0.2).reshape(B, C, Hg, Wg))
 
@@ -219,7 +228,7 @@ def _network_case(port, monkeypatch, mod_blocks, mode, Rh, Rw, seed):
         if pc[n].grad is None:         # e.g. the ToRGB layers of blocks 0-2, which the forward never uses
             assert pg[n].grad is None or float(pg[n].grad.abs().max()) == 0.0, n
             continue
-        assert pg[n].grad is not None, n
+        assert pg[n].grad is not None and pg[n].grad.shape == pg[n].shape, n
         a, b = pg[n].grad.cpu().double(), pc[n].grad.double()
         if b.norm().item() < 1e-9 * scale:      # analytic zeros (a conv bias in front of a BatchNorm)
             err = a.norm().item() / scale
@@ -237,10 +246,12 @@ def _network_case(port, monkeypatch, mod_blocks, mode, Rh, Rw, seed):
 
 
 def test_synthesis_network_backward_const_style(port, monkeypatch):
+    """Block 0 const-style at 256: its data gradient reads the batch-shared synthesis input."""
     _network_case(port, monkeypatch, [], "mixed", 4, 6, 5)
 
 
+@pytest.mark.parametrize("C", [256, 384, 420])
 @pytest.mark.parametrize("mode", ["mixed", "isolated"])
-def test_synthesis_network_backward_mixed(port, monkeypatch, mode):
+def test_synthesis_network_backward_mixed(port, monkeypatch, mode, C):
     """Blocks 0-2 pixel-style (per-pixel gamma/beta from the up-sampled render features), 3-8 const-style."""
-    _network_case(port, monkeypatch, [0, 1, 2], mode, 5, 7, 7)
+    _network_case(port, monkeypatch, [0, 1, 2], mode, 5, 7, 7, C)

@@ -1,14 +1,15 @@
-"""Training at hidden_dim 384 (MAP3DBN) and 420 (MAP3DBN512L): the zero-padded forward with a tape and its backward
-(modules/wide_train.py) against fp64 / fp32 autograd through the restated reference, from the data-gradient kernel's
-K = 512 operand scale up to `Trainer.iteration`."""
+"""Training at hidden_dim 384 (MAP3DBN) and 420 (MAP3DBN512L): the zero-padded forward with a tape and the backward
+every width shares, against fp64 / fp32 autograd through the restated reference, from the data-gradient kernel's
+K = 512 operand scale up to `Trainer.iteration`.  The renderer and synthesis backward at these widths are tested
+layer by layer next to the 256-channel cases: test_gpu_render_train.py::test_render_train_forward_and_backward (the
+renderer test the sigma-bias note below calls test_render_wide_forward_and_backward) and
+test_gpu_synthesis_bwd.py::test_synthesis_network_backward_mixed."""
 import importlib
 
 import pytest
 import torch
 
 pytestmark = pytest.mark.gpu
-
-WIDTHS = [384, 420]
 
 
 def _blocked(t):
@@ -23,11 +24,6 @@ def _blocked(t):
 def _planar(t, HW):
     B, T, Cc, _ = t.shape
     return t.permute(0, 2, 1, 3).reshape(B, Cc, T * 128)[:, :, :HW]
-
-
-def _halves_planar(pair, C, HW):
-    """Two tile-blocked halves [B,T,256,128] -> [B,C,HW] (padded channels dropped)."""
-    return torch.cat([_planar(p, HW) for p in pair], 1)[:, :C]
 
 
 def _rel(a, b):
@@ -75,164 +71,7 @@ def test_conv_bwd_operand_scale(act, K):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
-# 2. renderer
-# ----------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("C", WIDTHS)
-def test_render_wide_forward_and_backward(port, monkeypatch, C):
-    pkg = importlib.import_module("3dhumangan_b200")
-    rt = importlib.import_module("3dhumangan_b200.modules.render_train")
-    wo = importlib.import_module("3dhumangan_b200.modules.wide_ops")
-    wt = importlib.import_module("3dhumangan_b200.modules.wide_train")
-    B, R, S, seed = 2, 8, 32, 11
-    cfg = pkg.configs.baseline_config("tiny")
-    cfg.update(hidden_dim=C, feature_dim=C, num_steps=S, nerf_noise=0.5, white_back=True, last_back=False, clamp_mode="relu")
-    params = port.init_generator_params(cfg, seed=seed, sigma_gain=60.0, sigma_bias=2.0)
-    names = [n for n in params if n.startswith("neural_field.")]
-    g = torch.Generator().manual_seed(seed + 1)
-    N = R * S
-    pts = torch.rand(B, N, 3, generator=g) * 2 - 1
-    geo = torch.rand(B, N, 31, generator=g)
-    z = (torch.rand(B, R, S, generator=g) * 0.02 + 0.03).cumsum(-1) + 8.0
-    freq = torch.randn(B, 4 * C, generator=g)
-    phase = torch.randn(B, 4 * C, generator=g)
-    noise = torch.randn(B, R, S, 1, generator=g)
-    wgt = torch.randn(B, R, 3 + C, generator=g)
-
-    pg = {n: params[n].clone().cuda().requires_grad_(True) for n in names}
-    rec = torch.cat([pts, geo], -1).cuda()
-    monkeypatch.setattr(rt, "geo_records", lambda *a, **k: (rec, z.reshape(B, N).cuda().contiguous()))
-    tape = {}
-    feats, rgb01, _ = wo.render_forward_wide(pg, freq.cuda(), phase.cuda(), None, cfg, None, noise.cuda(), tape=tape)
-    dfq, dph = wt.render_backward_wide(tape, wgt[..., 3:].cuda(), wgt[..., :3].cuda())
-    torch.cuda.synchronize()
-
-    def oracle(mask):
-        pc = {n: params[n].clone().double().requires_grad_(True) for n in names}
-        fq, ph = freq.clone().double().requires_grad_(True), phase.clone().double().requires_grad_(True)
-        dirs = torch.zeros(B, N, 3, dtype=torch.float64)
-        dirs[..., -1] = -1
-        raw = port.siren(pc, pts.double(), fq, ph, geo.double(), dirs, 1.0, C, 4)
-        with monkeypatch.context() as mp:
-            if mask is not None:      # the sigma ReLU mask of the kernels (the gradient is discontinuous in it)
-                mp.setattr(port.F, "relu", lambda v: v * mask)
-            rgbf, _, _ = port.ray_integration(raw.reshape(B, R, S, -1), z.double()[..., None], noise.double(), cfg["nerf_noise"],
-                                              True, False, "relu")
-        return rgbf, pc, fq, ph
-
-    with torch.no_grad():
-        rgbf = oracle(None)[0]
-    assert (feats.cpu().double() - rgbf[..., 3:]).abs().max() / rgbf[..., 3:].abs().max() < 1e-3
-    assert (rgb01.cpu().double() - rgbf[..., :3]).abs().max() < 1e-3
-
-    mask = ((tape["sig"].cpu().double().reshape(B, R, S, 1) + noise.double() * cfg["nerf_noise"]) > 0).double()
-    assert 0.05 < mask.mean().item() < 0.95
-    rgbf, pc, fq, ph = oracle(mask)
-    (rgbf * wgt.double()).sum().backward()
-    bad = {}
-    for n in names:
-        assert pg[n].grad is not None and pg[n].grad.shape == pg[n].shape, n
-        e = _rel(pg[n].grad.cpu().double(), pc[n].grad)
-        if e > 1e-3:
-            bad[n] = e
-    assert not bad, sorted(bad.items(), key=lambda t: -t[1])
-    assert _rel(dfq.cpu().double(), fq.grad) < 1e-3
-    assert _rel(dph.cpu().double(), ph.grad) < 1e-3
-
-
-# ----------------------------------------------------------------------------------------------------------------------
-# 3. synthesis network
-# ----------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("C,mode,mod_blocks", [(384, "mixed", [0, 1, 2]), (420, "isolated", [0, 1, 2])])
-def test_synthesis_wide_backward(port, monkeypatch, C, mode, mod_blocks):
-    """As tests/test_gpu_synthesis_bwd.py::_network_case: the fp64 reference is evaluated with the LeakyReLU / ReLU masks
-    the kernels differentiate through; the forward is compared without help."""
-    import torch.nn.functional as TF
-    pkg = importlib.import_module("3dhumangan_b200")
-    st = importlib.import_module("3dhumangan_b200.modules.synthesis_train")
-    wo = importlib.import_module("3dhumangan_b200.modules.wide_ops")
-    wt = importlib.import_module("3dhumangan_b200.modules.wide_train")
-    Rh, Rw, seed = 5, 7, 7
-    cfg = pkg.configs.baseline_config("tiny")
-    cfg.update(hidden_dim=C, feature_dim=C, gen_height=16, gen_width=24, render_height=Rh, render_width=Rw, mod_blocks=mod_blocks,
-               map3d_mode=mode)
-    B, Hg, Wg = 2, 16, 24
-    HW = Hg * Wg
-    params = port.init_generator_params(cfg, seed=seed)
-    names = [n for n in params if n.startswith(("synthesis_network.", "synthesis_input."))]
-    learn = [n for n in names if not n.endswith(("weight_u", "weight_v", "running_mean", "running_var", "num_batches_tracked"))]
-    g = torch.Generator().manual_seed(seed + 1)
-    fixed = torch.randn(B, 1, C, generator=g) * 0.5
-    fmap = torch.randn(B, C, Rh, Rw, generator=g) * 0.7
-    wgt = torch.randn(B, 3, Hg, Wg, generator=g)
-
-    pg = {n: params[n].clone().cuda() for n in names}
-    for n in learn:
-        pg[n].requires_grad_(True)
-    feat_lr = fmap.permute(0, 2, 3, 1).reshape(B, Rh * Rw, C).contiguous().cuda()
-    tape = st.SynthesisTape()
-    rgb = wo.synthesis_forward_wide(pg, feat_lr, fixed.cuda(), cfg, training=True, tape=tape)
-    tape.keep_masks = True
-    dfs, dfeat = wt.synthesis_backward_wide(pg, tape, wgt.cuda())
-    torch.cuda.synchronize()
-    masks, relu_masks = [], []
-    for rec in tape.halves:
-        if rec["pixel"]:
-            mk = _halves_planar(rec["mask"], C, HW).cpu()
-            masks.append(torch.where(mk, 1.0, 0.2).double().reshape(B, C, Hg, Wg))
-            relu_masks.append(_planar(rec["mask_a1"], HW).cpu().double().reshape(B, 128, Hg, Wg))
-            continue
-        relu_masks.append(None)
-        xp = _halves_planar(rec["x"], C, HW).double().cpu()
-        m = torch.cat(rec["mod_d"], -1)[..., :C].double().cpu()
-        pre = xp * m[:, 0, :, None] + m[:, 1, :, None]
-        masks.append(torch.where(pre > 0, 1.0, 0.2).reshape(B, C, Hg, Wg))
-
-    def oracle(mask_list):
-        pc = {n: (params[n].clone().double() if params[n].is_floating_point() else params[n].clone()) for n in names}
-        for n in learn:
-            pc[n].requires_grad_(True)
-        fc = fixed.clone().double().requires_grad_(True)
-        fm = fmap.clone().double().requires_grad_(True)
-        ii, jj = torch.linspace(-1, 1, Hg).double(), torch.linspace(-1, 1, Wg).double()
-        coords = torch.stack([ii[:, None].expand(Hg, Wg), jj[None, :].expand(Hg, Wg)], 0)[None].repeat(B, 1, 1, 1)
-        x0 = torch.sin(TF.conv2d(coords, pc["synthesis_input.network.0.weight"], pc["synthesis_input.network.0.bias"]))
-        style = TF.interpolate(fm, (Hg, Wg), mode="bilinear")
-        with monkeypatch.context() as mp:
-            if mask_list is not None:
-                it = iter(mask_list)
-                mp.setattr(port.F, "leaky_relu", lambda v, slope: v * next(it))
-                rit, real_relu = iter(relu_masks), TF.relu
-
-                def relu(v):
-                    mk = next(rit)
-                    return real_relu(v) if mk is None else v * mk
-                mp.setattr(port.F, "relu", relu)
-            out = port.synthesis_network(pc, x0, style, fc, cfg, training=True)
-        return out, pc, fc, fm
-
-    with torch.no_grad():
-        rgb_plain = oracle(None)[0]
-    assert (rgb.cpu().double() - rgb_plain).abs().max() / rgb_plain.abs().max() < 2e-4
-    rgb_ref, pc, fc, fm = oracle(masks)
-    (rgb_ref * wgt.double()).sum().backward()
-    scale = max(pc[n].grad.norm().item() for n in learn if pc[n].grad is not None)
-    bad = {}
-    for n in learn:
-        if pc[n].grad is None:         # the ToRGB layers of blocks 0-2, which the forward never uses
-            assert pg[n].grad is None or float(pg[n].grad.abs().max()) == 0.0, n
-            continue
-        assert pg[n].grad is not None and pg[n].grad.shape == pg[n].shape, n
-        a, b = pg[n].grad.cpu().double(), pc[n].grad.double()
-        err = a.norm().item() / scale if b.norm().item() < 1e-9 * scale else _rel(a, b)
-        if err > 5e-4:
-            bad[n] = err
-    assert not bad, sorted(bad.items(), key=lambda t: -t[1])[:8]
-    assert _rel(dfs.cpu().double().reshape(-1), fc.grad.reshape(-1)) < 5e-4
-    assert _rel(dfeat.cpu().double(), fm.grad.permute(0, 2, 3, 1).reshape(B, Rh * Rw, C)) < 5e-4
-
-
-# ----------------------------------------------------------------------------------------------------------------------
-# 4. whole generator
+# 2. whole generator
 # ----------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("C,mode,legacy", [(384, "mixed", False), (420, "isolated", True)])
 def test_generator_wide_backward_matches_oracle(port, monkeypatch, C, mode, legacy):
@@ -335,7 +174,7 @@ def test_wide_surface_guards(port):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
-# 5. trainer
+# 3. trainer
 # ----------------------------------------------------------------------------------------------------------------------
 def test_trainer_map3dbn_amp(pkg):
     """MAP3DBN (384) at small shapes: fp16 autocast + GradScaler, four iterations including a do_r1 phase."""

@@ -30,9 +30,9 @@ rgb, tape = st.synthesis_forward_train(pg, None, fixed.cuda(), cfg)
 masks = []
 HW = Hg * Wg
 for rec in tape.halves:
-    x = rec["x"] if rec["x"].dim() == 4 else rec["x"][None].expand(B, -1, -1, -1)
+    x = rec["x"][0].expand(B, -1, -1, -1)          # one 256-channel half; the synthesis input is batch-shared
     xp = x.permute(0, 2, 1, 3).reshape(B, C, -1)[:, :, :HW].double().cpu()
-    m = rec["mod_d"].double().cpu()
+    m = rec["mod_d"][0].double().cpu()
     pre = xp * m[:, 0, :, None] + m[:, 1, :, None]
     masks.append(torch.where(pre > 0, 1.0, 0.2).reshape(B, C, Hg, Wg))
 if "--samemask" in sys.argv:
