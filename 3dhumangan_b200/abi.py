@@ -29,6 +29,9 @@ SIGNATURES = {
     "hg_knn_padded": (c_int, [c_int]),
     "hg_knn_prep": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "hg_geo_features": (c_int, [c_void_p] * 14 + [c_int] * 6 + [c_float, c_int] + [c_void_p] * 6),
+    "hg_sample_fine": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_float, c_int] + [c_void_p] * 4 + [c_int] * 4
+                       + [c_void_p] * 3),
+    "hg_merge_samples": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p] * 4),
     "hg_spade_conv": (c_int, [c_void_p, c_long, c_void_p, c_void_p, c_void_p, c_long] + [c_void_p] * 12 + [c_int] * 7 + [c_void_p]),
     "hg_bn_finalize": (c_int, [c_void_p, c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_float,
                                c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
@@ -270,6 +273,38 @@ def geo_features(cond_vertices, tpose, skeletons, vik, *, input_scaler, legacy_m
                                     int(bool(legacy_mode)), ptr(rec), ptr(z_vals), ptr(pts), ptr(near), ptr(d2),
                                     stream())
     return {"rec": rec, "z_vals": z_vals, "points": pts, "nearest": near, "nearest_d2": d2}
+
+
+def sample_fine(sigma, sigma_stride, z_vals, noise, u_pdf, *, noise_std, clamp_mode, xs, ys, focals, cam2world, B, Rw, Rh, S):
+    """Coarse weights + inverse-cdf sampling of hierarchical_sample (csrc/sample.cu) -> fine z [B,R*S], points [B,R*S,3].
+    `sigma` is read at p * sigma_stride for point p (the sigma column of a per-point output can be passed as a view)."""
+    dev = z_vals.device
+    if clamp_mode not in ("relu", "softplus"):
+        raise RuntimeError("Need to choose clamp mode")          # volume_rendering.py:31
+    f = lambda t: None if t is None else t.float().contiguous()
+    keep = [f(t) for t in (z_vals, noise, u_pdf, xs, ys, focals, cam2world)]
+    fine_z = torch.empty(B, Rw * Rh * S, dtype=torch.float32, device=dev)
+    pts = torch.empty(B, Rw * Rh * S, 3, dtype=torch.float32, device=dev)
+    if not sigma.is_cuda:
+        raise RuntimeError("hg3d: expected a CUDA tensor (there is no CPU path)")
+    with torch.cuda.device_of(fine_z):
+        call("hg_sample_fine", c_void_p(sigma.data_ptr()), int(sigma_stride), ptr(keep[0]), ptr(keep[1]), ptr(keep[2]),
+             float(noise_std), int(clamp_mode == "softplus"), *[ptr(t) for t in keep[3:]], B, Rw, Rh, S, ptr(fine_z), ptr(pts),
+             stream())
+    return fine_z, pts
+
+
+def merge_samples(fine_rec, fine_z, coarse_rec, coarse_z, *, B, R, S, want_perm=False):
+    """Depth-sorted merge of the fine and coarse samples of every ray (csrc/sample.cu) -> rec [B,R*2S,36], z [B,R*2S],
+    perm [B,R*2S] int32 (index into cat([fine, coarse]) per ray) or None."""
+    dev = fine_rec.device
+    rec = torch.empty(B, R * 2 * S, 36, dtype=torch.float32, device=dev)
+    z = torch.empty(B, R * 2 * S, dtype=torch.float32, device=dev)
+    perm = torch.empty(B, R * 2 * S, dtype=torch.int32, device=dev) if want_perm else None
+    with torch.cuda.device_of(rec):
+        call("hg_merge_samples", ptr(fine_rec), ptr(fine_z), ptr(coarse_rec), ptr(coarse_z), B, R, S, ptr(rec), ptr(z), ptr(perm),
+             stream())
+    return rec, z, perm
 
 
 def spade_conv(x, x_bstride, wimg, bias, out, *, B, Hg, Wg, mod=None, scsh=None, p_lr=None, p_stride=0, p_bias=None,

@@ -312,7 +312,7 @@ class Map3DGenerator(nn.Module):
 
     def _guard(self, kwargs):
         for key, bad in (("disable_render", True), ("disable_synthesis", True), ("2d_label_input", True),
-                         ("2d_latent_input", True), ("hierarchical_sample", True)):
+                         ("2d_latent_input", True)):
             if kwargs.get(key, False) == bad:
                 raise RuntimeError(f"hg3d: {key}={bad} is not used by any shipped curriculum and is not built")
         if kwargs.get("feature_map_interpolation", "bilinear") != "bilinear":
@@ -334,7 +334,7 @@ class Map3DGenerator(nn.Module):
         P = self._params()
         cond = {k: conditions[k] for k in ("skeletons_xyz", "vertices", "tpose_vertices", "fk_matrices", "lbs_weights",
                                            "cam2world_matrices", "intrinsics", "scales")}
-        u, noise = rng.draw_render_noise(B, Rh * Rw, S, dev, cfg.get("sample_dist", None))
+        u, noise = rng.draw(B, Rh * Rw, S, dev, cfg)
         if self.hidden_dim != 256 and not self._wants_grad():
             # hidden_dim 384 (MAP3DBN) / 420 (MAP3DBN512L, the released checkpoint): the zero-padded 2 x 256 path on the
             # general blocked-GEMM engine (modules/wide_ops.py); under autograd it runs inside GeneratorCore below

@@ -1,7 +1,7 @@
 """Host-side schedule of the pose-mapping renderer on top of the C ABI (csrc/geo.cu, csrc/render.cu).
 
-Mirrors `Map3DGenerator.render` (lib/generators/map3d_generator.py:381-523) for the shipped
-configuration space: hierarchical_sample=False, one coarse pass.  Three launches per call:
+Mirrors `Map3DGenerator.render` (lib/generators/map3d_generator.py:381-523) with lock_view_dependence=True.  Three
+launches per one-pass call (hierarchical_sample=True first builds 2S merged samples per ray, modules/hierarchical.py):
 `hg_vertex_ik` (inverse-LBS matrices per posed vertex), `hg_geo_features` (rays, jitter, camera
 transform, exact K=1 nearest vertex, 31-d feature) and `hg_render_mlp` (FiLM-SIREN + compositing).
 """
@@ -61,29 +61,34 @@ def film_table(P, freq, phase, locked_dir=(0.0, 0.0, -1.0), prefix="neural_field
 
 @torch.no_grad()
 def render_forward(P, freq, phase, cond, cfg, u, noise, *, passes=3, wblob=None, want_weights=False, want_nearest=False):
-    """u [B,R,S,1] jitter draws, noise [B,R,S,1] sigma-noise draws (rng.draw_render_noise).
-    Returns dict(ray_out [B,R,260], z_vals, weights, nearest)."""
+    """u [B,R,S,1] jitter draws, noise [B,R,S,1] sigma-noise draws (rng.draw_render_noise); with hierarchical_sample
+    `noise` is the rng.HierarchicalNoise of the render and the integration runs over the 2S merged samples
+    (modules/hierarchical.py).  Returns dict(ray_out [B,R,260], z_vals, weights, nearest)."""
     abi.require_device()
-    if cfg.get("hierarchical_sample", False):
-        raise RuntimeError("hg3d: hierarchical_sample=True is not used by any shipped curriculum and is not built")
     if not cfg.get("lock_view_dependence", False):
         raise RuntimeError("hg3d: lock_view_dependence=False is not used by any shipped curriculum and is not built")
     dev = freq.device
     B = freq.shape[0]
     Rw, Rh, S = cfg["render_width"], cfg["render_height"], cfg["num_steps"]
     R = Rw * Rh
-    f32 = dict(dtype=torch.float32, device=dev)
-    xs = torch.linspace(-Rw / Rh, Rw / Rh, Rw, **f32)
-    ys = torch.linspace(-1, 1, Rh, **f32)
-    zs = torch.linspace(cfg["ray_start"], cfg["ray_end"], S, **f32)
-    vik = abi.vertex_ik(cond["fk_matrices"], cond["lbs_weights"])
-    geo = abi.geo_features(cond["vertices"], cond["tpose_vertices"], cond["skeletons_xyz"], vik,
-                           input_scaler=2.0 / cfg["side_length"], legacy_mode=cfg.get("legacy_mode", False),
-                           xs=xs, ys=ys, zs=zs, focals=cond["intrinsics"][:, 0, 0], scales=cond["scales"],
-                           cam2world=cond["cam2world_matrices"], jitter=u.reshape(B, R * S) if u is not None else None,
-                           want_nearest=want_nearest)
     if wblob is None:
         wblob = pack_render_weights(P, geo_dim=cfg["geo_feature_dim"])
+    if cfg.get("hierarchical_sample", False):
+        from . import hierarchical
+        geo = hierarchical.merged_records(P, freq, phase, cond, cfg, u, noise, passes=passes, wblob=wblob,
+                                          want_nearest=want_nearest)
+        S, noise = 2 * S, geo["noise"]
+    else:
+        f32 = dict(dtype=torch.float32, device=dev)
+        xs = torch.linspace(-Rw / Rh, Rw / Rh, Rw, **f32)
+        ys = torch.linspace(-1, 1, Rh, **f32)
+        zs = torch.linspace(cfg["ray_start"], cfg["ray_end"], S, **f32)
+        vik = abi.vertex_ik(cond["fk_matrices"], cond["lbs_weights"])
+        geo = abi.geo_features(cond["vertices"], cond["tpose_vertices"], cond["skeletons_xyz"], vik,
+                               input_scaler=2.0 / cfg["side_length"], legacy_mode=cfg.get("legacy_mode", False),
+                               xs=xs, ys=ys, zs=zs, focals=cond["intrinsics"][:, 0, 0], scales=cond["scales"],
+                               cam2world=cond["cam2world_matrices"], jitter=u.reshape(B, R * S) if u is not None else None,
+                               want_nearest=want_nearest)
     film = film_table(P, freq, phase)
     g = lambda n: P["neural_field." + n]
     heads_b = torch.cat([g("sigma_layer.bias").reshape(1), g("color_layer_linear.bias").reshape(3)]).float().contiguous()

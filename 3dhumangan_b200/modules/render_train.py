@@ -290,8 +290,8 @@ class GeneratorCore(torch.autograd.Function):
             P[n] = t
         B = freq.shape[0]
         Rh, Rw = cfg["render_height"], cfg["render_width"]
-        if cfg.get("hierarchical_sample", False) or not cfg.get("lock_view_dependence", False):
-            raise RuntimeError("hg3d: the training renderer is built for hierarchical_sample=False, lock_view_dependence=True")
+        if not cfg.get("lock_view_dependence", False):
+            raise RuntimeError("hg3d: the training renderer is built for lock_view_dependence=True")
         if cfg.get("neural_field_blocks", 4) != 4:
             raise RuntimeError("hg3d: the training renderer is built for neural_field_blocks == 4 (all shipped curricula)")
         if cfg["hidden_dim"] != H:      # 384 / 420: the zero-padded forward of wide_ops, with tapes
@@ -301,9 +301,15 @@ class GeneratorCore(torch.autograd.Function):
             rgb = wide_ops.synthesis_forward_wide(P, feats, styles.reshape(B, -1), cfg, training=True, passes=passes, tape=stape)
             rgb_render = (rgb01 * 2 - 1).reshape(B, Rh, Rw, 3).permute(0, 3, 1, 2).contiguous()
         else:
-            rec, z_vals = geo_records(cond, cfg, u)
+            if cfg.get("hierarchical_sample", False):      # the 2S merged samples replace the ray stage's records
+                from . import hierarchical
+                h = hierarchical.merged_records(P, freq, phase, cond, cfg, u, noise, passes=passes)
+                rec, z_vals, rcfg, rnoise = h["rec"], h["z_vals"], h["cfg"], h["noise"]
+            else:
+                rec, z_vals = geo_records(cond, cfg, u)
+                rcfg, rnoise = cfg, noise
             with torch.enable_grad():
-                ray, rtape = mlp_forward_train(P, freq, phase, rec, z_vals, noise, cfg, geo_dim=cfg["geo_feature_dim"],
+                ray, rtape = mlp_forward_train(P, freq, phase, rec, z_vals, rnoise, rcfg, geo_dim=cfg["geo_feature_dim"],
                                                passes=passes)
                 rgb, stape = synthesis_train.synthesis_forward_train(P, ray, styles.reshape(B, -1), cfg, passes=passes)
             rgb_render = (ray[..., 256:259] * 2 - 1).reshape(B, Rh, Rw, 3).permute(0, 3, 1, 2).contiguous()

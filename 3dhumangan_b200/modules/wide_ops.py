@@ -82,11 +82,14 @@ def wide_layer(xs, W512, b512, *, mods=None, act=0, slope=0.2, skips=None, stats
 # renderer
 # ----------------------------------------------------------------------------------------------------------------------
 @torch.no_grad()
-def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix="neural_field.", tape=None):
+def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix="neural_field.", tape=None, records=None,
+                        sigma_only=False):
     """-> ray features [B,R,C], rgb [B,R,3] (in [0,1], before the *2-1), depth [B,R,1].
     `tape` (a dict) receives what `render_train.mlp_backward` needs, in the format its docstring describes: per half the
     linear outputs lin_a, lin_b, out_0..3, lin_c, feat, then sig, rgbp and the FiLM tables built from freq / phase
-    leaves with autograd history."""
+    leaves with autograd history.
+    `records` (rec [B,N,36], z_vals [B,N]) replaces the ray stage (hierarchical_sample: the merged samples, with
+    cfg["num_steps"] the samples per ray).  `sigma_only` stops after the sigma head and returns the raw sigma [B,N]."""
     from . import render_train
     abi.require_device()
     g = lambda n: P[prefix + n].detach().float()
@@ -98,11 +101,15 @@ def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix
         raise RuntimeError("hg3d: the renderer is built for neural_field_blocks == 4 (all shipped curricula)")
     if tape is not None and cfg.get("last_back", False):
         raise RuntimeError("hg3d: last_back=True is an inference-only setting (eval_last_back); the training renderer does not build it")
+    if records is None and cfg.get("hierarchical_sample", False):
+        from . import hierarchical
+        h = hierarchical.merged_records(P, freq, phase, cond, cfg, u, noise, passes=passes)
+        records, cfg, noise = (h["rec"], h["z_vals"]), h["cfg"], h["noise"]
     dev = freq.device
     B = freq.shape[0]
     S = cfg["num_steps"]
     geo_dim = cfg["geo_feature_dim"]
-    rec, z_vals = render_train.geo_records(cond, cfg, u)
+    rec, z_vals = render_train.geo_records(cond, cfg, u) if records is None else records
     N = rec.shape[1]
     R = N // S
     if N % 128:
@@ -153,6 +160,16 @@ def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix
         x = wide_layer(x, _pad2(g(f"network.{i}.layer.weight"), 2 * HALF, 2 * HALF), _pad1(g(f"network.{i}.layer.bias"), 2 * HALF),
                        mods=mods[i - 1], act=1, **kw)
     out3 = x
+    w_sigma = _pad1(g("sigma_layer.weight").reshape(-1), 2 * HALF)
+    heads_b = torch.cat([g("sigma_layer.bias").reshape(1), g("color_layer_linear.bias").reshape(3)]).contiguous()
+    if sigma_only:
+        # hg_render_heads also forms the rgb head from its `linc` operand; out3 stands in for it and that output is dropped
+        sig = None
+        for h in (0, 1):
+            s_h, _ = abi.render_heads(out3[h], out3[h], mods[3][h], w_sigma[h * HALF:(h + 1) * HALF].contiguous(),
+                                      torch.zeros(3, HALF, **f32), heads_b if h == 0 else torch.zeros_like(heads_b), B=B, N=N)
+            sig = s_h if sig is None else sig + s_h
+        return sig
     wcol = g("color_layer_sine.layer.weight")
     dvec = torch.tensor((0.0, 0.0, -1.0), **f32)            # locked view direction (map3d_generator.py:418-420)
     bcol = g("color_layer_sine.layer.bias") + wcol[:, :3] @ dvec
@@ -160,9 +177,7 @@ def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix
     feat = wide_layer(lin_c, _pad2(g("feature_layer_linear.weight"), 2 * HALF, 2 * HALF), _pad1(g("feature_layer_linear.bias"), 2 * HALF),
                       mods=mods[3], act=1, **kw)
     # heads: sigma = w_s . sin(f3 out3 + phi3) + b, rgb_pre = W_rgb . sin(f3 lin_c + phi3) + b, summed over the halves
-    w_sigma = _pad1(g("sigma_layer.weight").reshape(-1), 2 * HALF)
     w_rgb = _pad2(g("color_layer_linear.weight"), 3, 2 * HALF)
-    heads_b = torch.cat([g("sigma_layer.bias").reshape(1), g("color_layer_linear.bias").reshape(3)]).contiguous()
     sig = rgbp = None
     for h in (0, 1):
         s_h, r_h = abi.render_heads(out3[h], lin_c[h], mods[3][h], w_sigma[h * HALF:(h + 1) * HALF].contiguous(),

@@ -72,6 +72,26 @@ int hg_geo_features(const float* xs, const float* ys, const float* zs, const flo
                     int legacy_mode, float* rec, float* z_vals, float* points, int* nearest, float* nearest_d2,
                     void* stream);
 
+/* Importance sampling of hierarchical_sample=True (csrc/sample.cu).  One warp per ray.  Replaces the coarse
+ * vr.ray_integration weights (map3d_generator.py:450-454), vr.sample_pdf (volume_rendering.py:261-303, det=False) and
+ * the fine points origin + direction * z (map3d_generator.py:463-465):
+ *   sigma: raw coarse sigma (before noise) of point p at sigma[p * sigma_stride], p over [B,R*S];
+ *   z_vals [B,R*S] jittered coarse depths; noise [B,R*S] N(0,1) draws of the coarse integration or NULL;
+ *   u_pdf [B*R,S] uniform draws of sample_pdf; clamp_softplus 0 = relu, 1 = softplus;
+ *   xs [Rw], ys [Rh], focals [B], cam2world [B,4,4]: the ray tables of hg_geo_features;
+ *   fine_z [B,R*S], fine_points [B,R*S,3] out.  3 <= S <= 64. */
+int hg_sample_fine(const float* sigma, int sigma_stride, const float* z_vals, const float* noise, const float* u_pdf,
+                   float noise_std, int clamp_softplus, const float* xs, const float* ys, const float* focals,
+                   const float* cam2world, int B, int Rw, int Rh, int S, float* fine_z, float* fine_points, void* stream);
+
+/* Merge of the fine and coarse samples (map3d_generator.py:500-505): per ray the 2S depths of cat([fine, coarse]) in
+ * ascending order, the fine sample first on equal depths (a tie has delta 0), with their point records.
+ *   fine_rec / coarse_rec [B,R*S,36] (16-byte aligned), fine_z / coarse_z [B,R*S];
+ *   rec_out [B,R*2S,36], z_out [B,R*2S]; perm_out [B,R*2S] (int32, index into cat([fine, coarse])) or NULL.
+ *   1 <= S <= 64. */
+int hg_merge_samples(const float* fine_rec, const float* fine_z, const float* coarse_rec, const float* coarse_z, int B,
+                     int R, int S, float* rec_out, float* z_out, int* perm_out, void* stream);
+
 /* Fused FiLM-SIREN MLP + volume integration.  Replaces COORDCONCATSIREN.forward (modulated.py:41-75)
  * and vr.ray_integration (volume_rendering.py:12-56).
  *   rec [B,R*S,36]; z_vals [B,R*S]; noise [B,R*S] N(0,1) draws or NULL;
