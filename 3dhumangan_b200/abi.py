@@ -52,7 +52,7 @@ SIGNATURES = {
     "hg_render_heads_bwd": (c_int, [c_void_p] * 6 + [c_int, c_int, c_void_p]),
     "hg_render_composite": (c_int, [c_void_p] * 7 + [c_int, c_int, c_int, c_float, c_int, c_int, c_int, c_void_p]),
     "hg_blocked_conv_wide": (c_int, [c_void_p] * 4 + [c_int, c_float] + [c_void_p] * 9 + [c_int] * 4 + [c_void_p]),
-    "hg_render_composite_bwd": (c_int, [c_void_p] * 9 + [c_int, c_int, c_int, c_float, c_int, c_int, c_void_p]),
+    "hg_render_composite_bwd": (c_int, [c_void_p] * 9 + [c_int, c_int, c_int, c_float, c_int, c_int, c_int, c_void_p]),
     "hg_wgrad_blocked": (c_int, [c_void_p, c_void_p, c_long, c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
     "hg_spade_a1": (c_int, [c_void_p, c_long, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
     "hg_spade_pixel_pre": (c_int, [c_void_p, c_long, c_void_p, c_void_p, c_void_p] + [c_int] * 4 + [c_void_p]),
@@ -78,6 +78,7 @@ SIGNATURES = {
     "hg_label_histogram": (c_int, [c_void_p, c_long, c_int, c_void_p, c_void_p]),
     "hg_seg_ce_coef": (c_int, [c_void_p, c_void_p, c_int, c_double, c_void_p, c_void_p]),
     "hg_seg_ce": (c_int, [c_void_p] * 6 + [c_int, c_int, c_long, c_void_p]),
+    "hg_image_loss": (c_int, [c_void_p] * 6 + [c_int, c_long, c_int, c_float, c_void_p]),
     "hg_mt_entry_bytes": (c_int, []),
     "hg_mt_chunk_bytes": (c_int, []),
     "hg_mt_chunk_elems": (c_int, []),
@@ -409,13 +410,13 @@ def render_composite(sig, z, noise, rgbp, feat, *, B, R, S, noise_std, white_bac
     return ray_out, w
 
 
-def render_composite_bwd(sig, z, noise, rgbp, feat, dray, *, B, R, S, noise_std, white_back, softplus):
+def render_composite_bwd(sig, z, noise, rgbp, feat, dray, *, B, R, S, noise_std, white_back, softplus, last_back=False):
     dfeat = torch.empty_like(feat)
     drgbp = torch.empty_like(rgbp)
     dsig = torch.empty_like(sig)
     with torch.cuda.device_of(sig):
         call("hg_render_composite_bwd", ptr(sig), ptr(z), ptr(noise), ptr(rgbp), ptr(feat), ptr(dray), ptr(dfeat), ptr(drgbp),
-             ptr(dsig), B, R, S, float(noise_std), int(bool(white_back)), int(bool(softplus)), stream())
+             ptr(dsig), B, R, S, float(noise_std), int(bool(white_back)), int(bool(softplus)), int(bool(last_back)), stream())
     return dfeat, drgbp, dsig
 
 

@@ -122,6 +122,8 @@ __global__ void __launch_bounds__(256) heads_bwd_kernel(const float* __restrict_
 //   delta_s = z_{s+1} - z_s (1e9 for the last), dens = relu|softplus(sigma + eps*noise_std), alpha = 1 - exp(-delta*dens),
 //   T_s = prod_{k<s} (1 - alpha_k + 1e-12), w = alpha*T; out[c] = sum_s w_s v_s[c] (+ 1 - sum w if white_back);
 //   v = [feat(256), sigmoid(rgb_pre)(3)]; depth = sum (w_s + [s = S-1](1 - sum w)) z_s.
+//   last_back: w_{S-1} += 1 - sum w before the sums (volume_rendering.py:38-41), so with g = d out
+//   d v_{S-1} gains (1 - sum w) g and every d w_s gains -<g, v_{S-1}>; the suffix sums of d alpha are unchanged.
 // ray_out [B,R,260] = feat | rgb | depth, exactly the layout of the fused forward kernel (csrc/render.cu).
 // ---------------------------------------------------------------------------------------------------------
 struct CompArgs {
@@ -139,7 +141,7 @@ struct CompArgs {
   int B, R, S;
   float noise_std;
   int white_back, softplus;
-  int last_back;         // fwd only: the last sample of a ray absorbs the remaining transmittance (volume_rendering.py:38-41)
+  int last_back;         // the last sample of a ray absorbs the remaining transmittance (volume_rendering.py:38-41)
 };
 
 __device__ __forceinline__ float comp_alpha(const CompArgs& a, long gp, int s, const float* zs, int row, float& dens_grad) {
@@ -243,15 +245,19 @@ __global__ void __launch_bounds__(128) composite_kernel(CompArgs a) {
     for (int i = row; i < rpt * 260; i += 128) sdr[i] = a.dray[(static_cast<long>(b) * a.R + ray0) * 260 + i];
     __syncthreads();
     const float* dr = sdr + rl * 260;
-    // q = <dout, v - back> over the 259 composited channels
+    // q = d out / d w_s = <dout, v_s - back (- v_{S-1} with last_back)> over the 259 composited channels
+    const int last = rl * S + S - 1;
+    const float lb = a.last_back ? 1.f : 0.f;
     float q = 0.f;
 #pragma unroll 4
-    for (int c = 0; c < kRC; ++c) q = fmaf(dr[c], ft[c * 128 + row] - back, q);
+    for (int c = 0; c < kRC; ++c) q = fmaf(dr[c], ft[c * 128 + row] - back - lb * ft[c * 128 + last], q);
     float sgm[3];
 #pragma unroll
     for (int j = 0; j < 3; ++j) {
-      sgm[j] = 1.f / (1.f + expf(-a.rgbp[(static_cast<long>(b) * 3 + j) * N + ti * 128 + row]));
-      q = fmaf(dr[kRC + j], sgm[j] - back, q);
+      const float* rp = a.rgbp + (static_cast<long>(b) * 3 + j) * N + ti * 128;
+      sgm[j] = 1.f / (1.f + expf(-rp[row]));
+      const float vl = a.last_back ? 1.f / (1.f + expf(-rp[last])) : 0.f;
+      q = fmaf(dr[kRC + j], sgm[j] - back - vl, q);
     }
     qs[row] = q * w;
     __syncthreads();
@@ -259,11 +265,12 @@ __global__ void __launch_bounds__(128) composite_kernel(CompArgs a) {
     for (int k = s + 1; k < S; ++k) suffix += qs[rl * S + k];
     const float dalpha = q * Tr - suffix / tr[row];
     a.dsig[gp] = dalpha * dgrad;
+    const float wv = (a.last_back && s == S - 1) ? w + (1.f - rayw[rl]) : w;      // d out / d v_s
 #pragma unroll
-    for (int j = 0; j < 3; ++j) a.drgbp[(static_cast<long>(b) * 3 + j) * N + ti * 128 + row] = w * dr[kRC + j] * sgm[j] * (1.f - sgm[j]);
+    for (int j = 0; j < 3; ++j) a.drgbp[(static_cast<long>(b) * 3 + j) * N + ti * 128 + row] = wv * dr[kRC + j] * sgm[j] * (1.f - sgm[j]);
     float* df = a.dfeat + static_cast<long>(tile) * kRC * 128 + row;
 #pragma unroll 4
-    for (int c = 0; c < kRC; ++c) df[c * 128] = w * dr[c];
+    for (int c = 0; c < kRC; ++c) df[c * 128] = wv * dr[c];
   }
 }
 
@@ -313,13 +320,14 @@ int hg_render_composite(const float* sig, const float* z, const float* noise, co
 
 int hg_render_composite_bwd(const float* sig, const float* z, const float* noise, const float* rgbp, const float* feat,
                             const float* dray, float* dfeat, float* drgbp, float* dsig, int B, int R, int S,
-                            float noise_std, int white_back, int clamp_softplus, void* stream) {
+                            float noise_std, int white_back, int clamp_softplus, int last_back, void* stream) {
   HG_REQUIRE(sig && z && rgbp && feat && dray && dfeat && drgbp && dsig, "hg_render_composite_bwd: null pointer");
   if (int rc = comp_check(B, R, S, "hg_render_composite_bwd")) return rc;
   hg::CompArgs a{};
   a.sig = sig; a.z = z; a.noise = noise; a.rgbp = rgbp; a.feat = feat; a.dray = dray; a.dfeat = dfeat; a.drgbp = drgbp;
   a.dsig = dsig;
   a.B = B; a.R = R; a.S = S; a.noise_std = noise_std; a.white_back = white_back; a.softplus = clamp_softplus;
+  a.last_back = last_back;
   hg::composite_kernel<true><<<B * (R * S / 128), 128, 0, static_cast<cudaStream_t>(stream)>>>(a);
   return hg::check_launch("hg_render_composite_bwd");
 }

@@ -256,7 +256,7 @@ __global__ void wgrad_reduce_kernel(const float* __restrict__ part_w, const floa
 // ------------------------------------------------------------------------------------------
 struct CombineArgs {
   const float* dpre;     // [B,T,C,128] or null (then only the skip / rgb terms)
-  const float* x;        // [B or 1,T,C,128] (needed when k or rgb_w is given)
+  const float* x;        // [B or 1,T,C,128] (read only when k or dwrgb is given)
   long x_bstride;
   const float* g1;       // [B,2,C] (row 0 used) or null
   const float* ak;       // [2,C]: a, k or null
@@ -299,7 +299,7 @@ __global__ void __launch_bounds__(256) spade_combine_kernel(CombineArgs a) {
     for (int c = warp; c < kWC; c += 8) {
       float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
       float4 xv = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (a.ak || a.drgb) xv = __ldcs(reinterpret_cast<const float4*>(a.x + xoff + c * 128));
+      if (a.ak || a.dwrgb) xv = __ldcs(reinterpret_cast<const float4*>(a.x + xoff + c * 128));
       if (a.dpre) {
         const float4 d = __ldcs(reinterpret_cast<const float4*>(a.dpre + off + c * 128));
         const float g = a.g1[static_cast<long>(b) * 2 * kWC + c];
@@ -659,7 +659,7 @@ int hg_spade_bwd_combine(const float* dpre, const float* x, long x_bstride, cons
   HG_REQUIRE(C == hg::kWC, "hg_spade_bwd_combine: only %d channels are supported (got %d)", hg::kWC, C);
   HG_REQUIRE(dx, "hg_spade_bwd_combine: null output");
   HG_REQUIRE(!dpre || g1, "hg_spade_bwd_combine: dpre needs its g1 table");
-  HG_REQUIRE(!(ak || drgb) || x, "hg_spade_bwd_combine: x is needed for the statistics / ToRGB terms");
+  HG_REQUIRE(!(ak || dwrgb) || x, "hg_spade_bwd_combine: x is needed for the statistics / ToRGB weight-gradient terms");
   HG_REQUIRE(!drgb || rgb_w, "hg_spade_bwd_combine: drgb needs rgb_w");
   HG_REQUIRE(!drgb || ((Hg * Wg) % 4 == 0 && (reinterpret_cast<uintptr_t>(drgb) & 15) == 0),
              "hg_spade_bwd_combine: drgb must be 16-byte aligned with H*W a multiple of 4");

@@ -116,6 +116,40 @@ __global__ void sum_partials_kernel(const double* __restrict__ partials, int n, 
 }
 
 // ------------------------------------------------------------------------------------------------------------------
+// image reconstruction loss: mean over the B*3*HW elements of m[b,p] * rho(pred - target), rho(d) = d^2 (mode 0) or the
+// Charbonnier sqrt(d^2 + eps^2) (mode 1; eps -> 0 is L1), and its gradient, in one pass.  fp64 partial per block.
+// ------------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) image_loss_kernel(const float* __restrict__ pred, const float* __restrict__ target,
+                                                         const float* __restrict__ mask, int mode, float eps, float scale,
+                                                         float* __restrict__ dpred, double* __restrict__ partials, long total,
+                                                         long HW) {
+  __shared__ double red[8];
+  double acc = 0.0;
+  for (long e = static_cast<long>(blockIdx.x) * blockDim.x + threadIdx.x; e < total; e += static_cast<long>(gridDim.x) * blockDim.x) {
+    const float d = __ldcs(pred + e) - __ldcs(target + e);
+    const float m = mask ? __ldg(mask + (e / (3 * HW)) * HW + e % HW) : 1.f;
+    float rho, drho;
+    if (mode == 0) {
+      rho = d * d;
+      drho = 2.f * d;
+    } else {
+      rho = sqrtf(fmaf(d, d, eps * eps));
+      drho = d / rho;
+    }
+    acc += static_cast<double>(m * rho);
+    if (dpred) __stcs(dpred + e, m * drho * scale);
+  }
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+    for (int i = 0; i < 8; ++i) t += red[i];
+    partials[blockIdx.x] = t;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
 // multi-tensor clip / Adam / EMA
 // ------------------------------------------------------------------------------------------------------------------
 struct MtEntry {          // 48 bytes
@@ -243,6 +277,25 @@ int hg_seg_ce(const float* logits, const long* labels, const float* coef, float*
   if (rc) return rc;
   hg::sum_partials_kernel<<<1, 1, 0, st>>>(workspace, static_cast<int>(blocks), 1.0 / static_cast<double>(total), loss);
   return hg::check_launch("hg_seg_ce(reduce)");
+}
+
+// loss[0] = mean over the B*3*HW elements of mask[b,p] * rho(pred - target); dpred (optional) = d loss / d pred.  The block
+// partials are summed by one thread in block order, so the value repeats bit for bit.  workspace: >= 8 * (2 * #SMs) bytes.
+int hg_image_loss(const float* pred, const float* target, const float* mask, float* dpred, float* loss, double* workspace,
+                  int B, long HW, int mode, float eps, void* stream) {
+  HG_REQUIRE(pred && target && loss && workspace, "hg_image_loss: null pointer");
+  HG_REQUIRE(B > 0 && HW > 0, "hg_image_loss: bad shape");
+  HG_REQUIRE(mode == 0 || (mode == 1 && eps > 0.f), "hg_image_loss: mode 0 (L2) or 1 (Charbonnier, eps > 0)");
+  auto st = static_cast<cudaStream_t>(stream);
+  const long total = static_cast<long>(B) * 3 * HW;
+  long blocks = (total + 255) / 256;
+  if (blocks > hg::num_sms() * 2) blocks = hg::num_sms() * 2;
+  hg::image_loss_kernel<<<static_cast<unsigned>(blocks), 256, 0, st>>>(pred, target, mask, mode, eps, 1.f / static_cast<float>(total),
+                                                                      dpred, workspace, total, HW);
+  int rc = hg::check_launch("hg_image_loss");
+  if (rc) return rc;
+  hg::sum_partials_kernel<<<1, 1, 0, st>>>(workspace, static_cast<int>(blocks), 1.0 / static_cast<double>(total), loss);
+  return hg::check_launch("hg_image_loss(reduce)");
 }
 
 int hg_mt_entry_bytes(void) { return static_cast<int>(sizeof(hg::MtEntry)); }

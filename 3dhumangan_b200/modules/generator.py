@@ -12,8 +12,10 @@ reference's ~150 ATen launches:
     hg_spade_conv x18 SPADE half-blocks with BatchNorm / modulation / ToRGB fused around wgmma GEMMs
 
 There is no CPU or eager-PyTorch fallback: without a CUDA device and lib3dhg_sm90a.so the
-forward raises RuntimeError.  With autograd enabled on parameters that require grad, `forward` runs the
-training kernels (modules/render_train.py, modules/synthesis_train.py) and its outputs are differentiable.
+forward raises RuntimeError.  With autograd enabled on parameters or inputs that require grad, `forward` runs the
+training kernels (modules/render_train.py, modules/synthesis_train.py) and its outputs are differentiable: in
+train() mode with batch statistics, in eval() mode with the running statistics and no buffer written (latent
+inversion through `synthesize`, fine-tuning with frozen statistics).
 """
 from __future__ import annotations
 
@@ -307,8 +309,10 @@ class Map3DGenerator(nn.Module):
     def _params(self):
         return OrderedDict(list(self.named_parameters()) + list(self.named_buffers()))
 
-    def _wants_grad(self):
-        return torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())
+    def _wants_grad(self, *inputs):
+        """Autograd is on and a parameter or one of `inputs` (a frozen generator asked for d / d latent) requires grad."""
+        return torch.is_grad_enabled() and (any(p.requires_grad for p in self.parameters())
+                                            or any(t is not None and t.requires_grad for t in inputs))
 
     def _guard(self, kwargs):
         for key, bad in (("disable_render", True), ("disable_synthesis", True), ("2d_label_input", True),
@@ -327,7 +331,8 @@ class Map3DGenerator(nn.Module):
         cfg.setdefault("num_steps", 24)
         return cfg
 
-    def _run(self, freq, phase, styles, conditions, cfg, passes):
+    def _run(self, freq, phase, styles, conditions, cfg, passes, want_records=False):
+        """-> (rgbs, rgbs_render, depth); with `want_records` (differentiable path only) also the render's (rec, z_vals)."""
         B = freq.shape[0]
         dev = freq.device
         Rh, Rw, S = cfg["render_height"], cfg["render_width"], cfg["num_steps"]
@@ -335,7 +340,11 @@ class Map3DGenerator(nn.Module):
         cond = {k: conditions[k] for k in ("skeletons_xyz", "vertices", "tpose_vertices", "fk_matrices", "lbs_weights",
                                            "cam2world_matrices", "intrinsics", "scales")}
         u, noise = rng.draw(B, Rh * Rw, S, dev, cfg)
-        if self.hidden_dim != 256 and not self._wants_grad():
+        wants_grad = self._wants_grad(freq, phase, styles)
+        if (want_records or cfg.get("hg_records") is not None) and not wants_grad:
+            raise RuntimeError("hg3d: hg_records re-uses the point records of a differentiable render; the inference kernels "
+                               "rebuild them in the fused pass")
+        if self.hidden_dim != 256 and not wants_grad:
             # hidden_dim 384 (MAP3DBN) / 420 (MAP3DBN512L, the released checkpoint): the zero-padded 2 x 256 path on the
             # general blocked-GEMM engine (modules/wide_ops.py); under autograd it runs inside GeneratorCore below
             from . import wide_ops
@@ -343,15 +352,15 @@ class Map3DGenerator(nn.Module):
             rgb = wide_ops.synthesis_forward_wide(P, feats, styles.reshape(B, -1), cfg, training=self.training, passes=passes)
             rgb_render = (rgb01 * 2 - 1).reshape(B, Rh, Rw, 3).permute(0, 3, 1, 2)
             return rgb, rgb_render, depth
-        if self._wants_grad():
-            # training step of the generator: layer-by-layer renderer + taped synthesis network (render_train.py,
-            # synthesis_train.py); the fused inference kernels below keep nothing for a backward pass
+        if wants_grad:
+            # training step of the generator, or gradients through it in eval mode: layer-by-layer renderer + taped
+            # synthesis network (render_train.py, synthesis_train.py); the fused inference kernels below keep nothing
+            # for a backward pass
             from . import render_train
-            if not self.training:
-                raise RuntimeError("hg3d: gradients through the generator are built for train() mode (batch statistics)")
             names, tensors = render_train.core_parameters(self)
-            return render_train.GeneratorCore.apply(self, cond, cfg, u, noise, passes, names, freq, phase,
-                                                    styles.reshape(B, -1), *tensors)
+            rgb, rgb_render, depth, rec, z_vals = render_train.GeneratorCore.apply(self, cond, cfg, u, noise, passes, names, freq,
+                                                                                   phase, styles.reshape(B, -1), *tensors)
+            return (rgb, rgb_render, depth, (rec, z_vals)) if want_records else (rgb, rgb_render, depth)
         r = render_ops.render_forward(P, freq, phase, cond, cfg, u, noise, passes=passes)
         ray = r["ray_out"]                                                   # [B,R,260]
         rgb = synthesis_ops.synthesis_forward(P, ray, styles.reshape(B, -1), cfg, training=self.training, passes=passes)
@@ -413,7 +422,7 @@ class Map3DGenerator(nn.Module):
         With autograd enabled and parameters that require grad (the generator step of the trainer) the training
         kernels run instead (render_train.GeneratorCore): outputs carry a grad_fn, `loss.backward()` fills `.grad`."""
         self._guard(kwargs)
-        if self._wants_grad():
+        if self._wants_grad(latent):
             cfg = self._cfg_for(kwargs, render_height, render_width)
             if latent_indices is not None:
                 latent = self.latent_pool(latent_indices)
@@ -443,6 +452,22 @@ class Map3DGenerator(nn.Module):
                     rgb, rgb_render, _ = self._forward_eager(latent, conditions, cfg, passes)
             else:
                 rgb, rgb_render, _ = self._forward_eager(latent, conditions, cfg, passes)
+        return {"rgbs": rgb, "rgbs_render": rgb_render}
+
+    def synthesize(self, freq, phase, styles, conditions, render_height, render_width, **kwargs):
+        """`forward` from the mapped space: freq / phase [B, 4*hidden_dim] of `neural_field_mapping_network`, styles
+        [B,1,feature_dim] of `synthesis_mapping_network` -> the dict of `forward`, differentiable in the three tensors
+        (truncation and mapped-space optimisation are the caller's).  Under autograd the dict also holds `hg_records`, the
+        point records (rec, z_vals) of this render: passed back as `hg_records=` they replace ray sampling, nearest-vertex
+        search and geometry features of a later call with the same pose, camera and jitter (they carry no gradient)."""
+        self._guard(kwargs)
+        cfg = self._cfg_for(kwargs, render_height, render_width)
+        if self._wants_grad(freq, phase, styles):
+            rgb, rgb_render, _, records = self._run(freq, phase, styles, conditions, cfg, _precision_passes(kwargs),
+                                                    want_records=True)
+            return {"rgbs": rgb, "rgbs_render": rgb_render, "hg_records": records}
+        with torch.no_grad():
+            rgb, rgb_render, _ = self._run(freq, phase, styles, conditions, cfg, _precision_passes(kwargs))
         return {"rgbs": rgb, "rgbs_render": rgb_render}
 
     def staged_forward(self, latent, conditions, render_height, render_width, truncation_psi, **kwargs):

@@ -42,16 +42,17 @@ def blocked_points(t, C):
 
 
 def mlp_forward_train(P, freq, phase, rec, z_vals, noise, cfg, *, geo_dim=31, locked_dir=(0.0, 0.0, -1.0), passes=3,
-                      prefix="neural_field."):
+                      prefix="neural_field.", training=True):
     """rec [B,N,>=3+geo_dim] (scaled coordinates, geometry features), z_vals [B,N], noise [B,N] or None.
-    Returns (ray_out [B,R,260] without autograd history, tape)."""
+    Returns (ray_out [B,R,260] without autograd history, tape).  `last_back=True` is differentiated for an eval-mode
+    module only (`training=False`): it is the sample app's compositing rule, no curriculum trains with it."""
     abi.require_device()
     g = lambda n: P[prefix + n]
     dev = rec.device
     B, N = rec.shape[0], rec.shape[1]
     S = cfg["num_steps"]
     R = N // S
-    if cfg.get("last_back", False):
+    if training and cfg.get("last_back", False):
         raise RuntimeError("hg3d: last_back=True is an inference-only setting (eval_last_back); the training renderer does not build it")
     if g("network.0.layer.weight").shape[0] != H:
         raise RuntimeError("hg3d: the sm_90a render kernels are built for hidden_dim == 256")
@@ -92,7 +93,7 @@ def mlp_forward_train(P, freq, phase, rec, z_vals, noise, cfg, *, geo_dim=31, lo
     sig, rgbp = abi.render_heads(outs[3], lin_c, mods[3], w_sigma, w_rgb, heads_b, B=B, N=N)
     noise = None if noise is None else noise.reshape(B, N).float().contiguous()
     comp = dict(B=B, R=R, S=S, noise_std=cfg["nerf_noise"], white_back=cfg.get("white_back", False),
-                softplus=cfg["clamp_mode"] == "softplus")
+                softplus=cfg["clamp_mode"] == "softplus", last_back=cfg.get("last_back", False))
     ray_out, _ = abi.render_composite(sig, z_vals, noise, rgbp, feat, **comp)
     tape = dict(P=P, prefix=prefix, C=H, Fd=H, geo_dim=geo_dim, fq=fq, ph=ph, mods=[(m,) for m in mods], mods_h=[(m,) for m in mods_h],
                 m30=(mod30,), rec_b=rec_b, lin_a=(lin_a,), lin_b=(lin_b,), outs=[(o,) for o in outs], lin_c=(lin_c,), feat=(feat,),
@@ -117,6 +118,7 @@ def mlp_backward(tape, dfeat, drgb, grads=None):
     from .synthesis_train import _packT, grad_accumulator
     P, prefix = tape["P"], tape["prefix"]
     g = lambda n: P[prefix + n]
+    need = lambda *names: any(g(n).requires_grad for n in names)      # a weight-gradient kernel runs only for these
     acc_ = grad_accumulator(P, grads)
     acc = lambda n, gr: acc_(prefix + n, gr)
     B, N, C, Fd, kw = tape["B"], tape["N"], tape["C"], tape["Fd"], tape["kw"]
@@ -148,11 +150,12 @@ def mlp_backward(tape, dfeat, drgb, grads=None):
         dsig = ds if dsig is None else dsig + ds
         del dray
     # ---- heads (the biases once)
-    hb = [abi.render_heads_bwd(outs[3][h], lin_c[h], mods[3][h], dsig, drgbp, B=B, N=N) for h in halves]
-    acc("sigma_layer.weight", torch.cat([t[:H] for t in hb])[:C].float())
-    acc("color_layer_linear.weight", torch.cat([t[H:4 * H].reshape(3, H) for t in hb], -1)[:, :C].float())
-    acc("sigma_layer.bias", hb[0][4 * H:4 * H + 1].float())
-    acc("color_layer_linear.bias", hb[0][4 * H + 1:].float())
+    if need("sigma_layer.weight", "color_layer_linear.weight", "sigma_layer.bias", "color_layer_linear.bias"):
+        hb = [abi.render_heads_bwd(outs[3][h], lin_c[h], mods[3][h], dsig, drgbp, B=B, N=N) for h in halves]
+        acc("sigma_layer.weight", torch.cat([t[:H] for t in hb])[:C].float())
+        acc("color_layer_linear.weight", torch.cat([t[H:4 * H].reshape(3, H) for t in hb], -1)[:, :C].float())
+        acc("sigma_layer.bias", hb[0][4 * H:4 * H + 1].float())
+        acc("color_layer_linear.bias", hb[0][4 * H + 1:].float())
 
     dmods = [[torch.zeros(B, 2, H, **f32) for _ in halves] for _ in range(4)]
 
@@ -186,44 +189,55 @@ def mlp_backward(tape, dfeat, drgb, grads=None):
     # ---- feature layer: feat = Wf sin(f3 lin_c + phi3) + bf;  the rgb head feeds back through the same activation (rank 3)
     dpre_c = dgrad(dfh, lin_c, _pad2(g("feature_layer_linear.weight").detach().float(), W, W), mods[3], film=3,
                    rk_w=tape["w_rgb"], rk_v=drgbp)
-    dW, db = wgrad(dfh, lin_c, mods[3], None)
-    acc("feature_layer_linear.weight", dW[:Fd, :C])
-    acc("feature_layer_linear.bias", db[:Fd])
+    if need("feature_layer_linear.weight", "feature_layer_linear.bias"):
+        dW, db = wgrad(dfh, lin_c, mods[3], None)
+        acc("feature_layer_linear.weight", dW[:Fd, :C])
+        acc("feature_layer_linear.bias", db[:Fd])
     del dfh
     # ---- colour layer: lin_c = Wcol' sin(f3 out3 + phi3) + bcol';  the sigma head feeds back through h4 (rank 1)
     wcol = g("color_layer_sine.layer.weight")
     dpre = dgrad(dpre_c, outs[3], _pad2(wcol[:, 3:].detach().float(), W, W), mods[3], film=3, ascale=scale(mods[3]),
                  rk_w=rk1, rk_v=dsig.reshape(B, 1, N))
-    dW, db = wgrad(dpre_c, outs[3], mods[3], pscale(mods[3]))
-    gw = torch.zeros_like(wcol)
-    gw[:, 3:] = dW[:C, :C]
-    acc("color_layer_sine.layer.weight", gw)
-    small = [(tape["bcol"], db[:C])]                                          # bias + direction columns via autograd
+    small = []
+    if need("color_layer_sine.layer.weight", "color_layer_sine.layer.bias"):
+        dW, db = wgrad(dpre_c, outs[3], mods[3], pscale(mods[3]))
+        gw = torch.zeros_like(wcol)
+        gw[:, 3:] = dW[:C, :C]
+        acc("color_layer_sine.layer.weight", gw)
+        small = [(tape["bcol"], db[:C])]                                      # bias + direction columns via autograd
     del dpre_c
     # ---- network.3 .. network.1: out_i = W_i sin(f_{i-1} out_{i-1} + phi_{i-1}) + b_i
     for i in (3, 2, 1):
         wi = _pad2(g(f"network.{i}.layer.weight").detach().float(), W, W)
         nxt = dgrad(dpre, outs[i - 1], wi, mods[i - 1], film=i - 1, ascale=scale(mods[i]))
-        dW, db = wgrad(dpre, outs[i - 1], mods[i - 1], pscale(mods[i]))
-        acc(f"network.{i}.layer.weight", dW[:C, :C])
-        acc(f"network.{i}.layer.bias", db[:C])
+        if need(f"network.{i}.layer.weight", f"network.{i}.layer.bias"):
+            dW, db = wgrad(dpre, outs[i - 1], mods[i - 1], pscale(mods[i]))
+            acc(f"network.{i}.layer.weight", dW[:C, :C])
+            acc(f"network.{i}.layer.bias", db[:C])
         dpre = nxt
     # ---- network.0 (K = 2C: coordinate part, geometry part) and the two first layers
     w0 = g("network.0.layer.weight").detach().float()
     gw0 = torch.empty(C, 2 * C, **f32)
+    need0 = need("network.0.layer.weight", "network.0.layer.bias")
     for part, lin, first, cols in ((0, tape["lin_a"], "first_layer_coord.layer.", slice(0, 3)),
                                    (1, tape["lin_b"], "first_layer_mod.layer.", slice(3, 3 + tape["geo_dim"]))):
-        dlin = dgrad(dpre, lin, _pad2(w0[:, part * C:(part + 1) * C], W, W), m30, ascale=scale(mods[0]))
-        dW, db0 = wgrad(dpre, lin, m30, pscale(mods[0]))
-        gw0[:, part * C:(part + 1) * C] = dW[:C, :C]
+        need_first = need(first + "weight", first + "bias")      # the coordinates and geometry features carry no gradient
+        if need_first:
+            dlin = dgrad(dpre, lin, _pad2(w0[:, part * C:(part + 1) * C], W, W), m30, ascale=scale(mods[0]))
+        if need0:
+            dW, db0 = wgrad(dpre, lin, m30, pscale(mods[0]))
+            gw0[:, part * C:(part + 1) * C] = dW[:C, :C]
+        if not need_first:
+            continue
         # first layer: lin = W x + b with the sine's factor 30 folded into the incoming gradient
         dwf, dbf = zip(*[abi.act_wgrad_blocked(dlin[h], tape["rec_b"], T * 128 * 128, None, act=2, pscale=m30[h][:, 0].contiguous(),
                                                Cx=128, **kw) for h in halves])
         acc(first + "weight", torch.cat(dwf)[:C, cols])
         acc(first + "bias", torch.cat(dbf)[:C])
         del dlin
-    acc("network.0.layer.weight", gw0)
-    acc("network.0.layer.bias", db0[:C])
+    if need0:
+        acc("network.0.layer.weight", gw0)
+        acc("network.0.layer.bias", db0[:C])
     # ---- FiLM tables, colour bias / direction columns: tiny autograd graphs
     outs_ = [t for m in tape["mods_h"] for t in m]
     grads_ = [t for m in dmods for t in m]
@@ -272,7 +286,8 @@ def core_parameters(module):
 
 
 class GeneratorCore(torch.autograd.Function):
-    """(freq, phase, fixed style, *renderer and synthesis parameters) -> (rgbs, rgbs_render, depth) on the sm_90a kernels.
+    """(freq, phase, fixed style, *renderer and synthesis parameters) -> (rgbs, rgbs_render, depth, rec, z_vals) on the sm_90a
+    kernels; rec / z_vals are the point records of the render (no gradient), which `cfg["hg_records"]` of a later call re-uses.
 
     EVERY parameter the kernels read is an input of this node and its gradient is RETURNED by `backward`, so the
     reference trainer's machinery sees them like any other autograd node's: `DistributedDataParallel` reducer hooks fire
@@ -294,34 +309,43 @@ class GeneratorCore(torch.autograd.Function):
             raise RuntimeError("hg3d: the training renderer is built for lock_view_dependence=True")
         if cfg.get("neural_field_blocks", 4) != 4:
             raise RuntimeError("hg3d: the training renderer is built for neural_field_blocks == 4 (all shipped curricula)")
+        training = module.training      # eval: running statistics, stored u / v, last_back allowed, no buffer written
+        # the point records: the 2S merged samples of hierarchical_sample, the ray stage's, or a previous render's
+        if cfg.get("hierarchical_sample", False):
+            if cfg.get("hg_records") is not None:
+                raise RuntimeError("hg3d: hg_records cannot be re-used with hierarchical_sample=True (the fine samples "
+                                   "follow the density, which moves with freq / phase)")
+            from . import hierarchical
+            h = hierarchical.merged_records(P, freq, phase, cond, cfg, u, noise, passes=passes)
+            rec, z_vals, rcfg, rnoise = h["rec"], h["z_vals"], h["cfg"], h["noise"]
+        else:
+            rec, z_vals = cfg["hg_records"] if cfg.get("hg_records") is not None else geo_records(cond, cfg, u)
+            rcfg, rnoise = cfg, noise
+        if rec.shape[:2] != (B, Rh * Rw * rcfg["num_steps"]) or z_vals.shape != rec.shape[:2]:
+            raise RuntimeError("hg3d: hg_records do not belong to this batch / render size / num_steps")
         if cfg["hidden_dim"] != H:      # 384 / 420: the zero-padded forward of wide_ops, with tapes
             from . import wide_ops
             rtape, stape = {}, synthesis_train.SynthesisTape()
-            feats, rgb01, depth = wide_ops.render_forward_wide(P, freq, phase, cond, cfg, u, noise, passes=passes, tape=rtape)
-            rgb = wide_ops.synthesis_forward_wide(P, feats, styles.reshape(B, -1), cfg, training=True, passes=passes, tape=stape)
+            feats, rgb01, depth = wide_ops.render_forward_wide(P, freq, phase, cond, rcfg, u, rnoise, passes=passes, tape=rtape,
+                                                               records=(rec, z_vals), training=training)
+            rgb = wide_ops.synthesis_forward_wide(P, feats, styles.reshape(B, -1), cfg, training=training, passes=passes, tape=stape)
             rgb_render = (rgb01 * 2 - 1).reshape(B, Rh, Rw, 3).permute(0, 3, 1, 2).contiguous()
         else:
-            if cfg.get("hierarchical_sample", False):      # the 2S merged samples replace the ray stage's records
-                from . import hierarchical
-                h = hierarchical.merged_records(P, freq, phase, cond, cfg, u, noise, passes=passes)
-                rec, z_vals, rcfg, rnoise = h["rec"], h["z_vals"], h["cfg"], h["noise"]
-            else:
-                rec, z_vals = geo_records(cond, cfg, u)
-                rcfg, rnoise = cfg, noise
             with torch.enable_grad():
                 ray, rtape = mlp_forward_train(P, freq, phase, rec, z_vals, rnoise, rcfg, geo_dim=cfg["geo_feature_dim"],
-                                               passes=passes)
-                rgb, stape = synthesis_train.synthesis_forward_train(P, ray, styles.reshape(B, -1), cfg, passes=passes)
+                                               passes=passes, training=training)
+                rgb, stape = synthesis_train.synthesis_forward_train(P, ray, styles.reshape(B, -1), cfg, passes=passes,
+                                                                     training=training)
             rgb_render = (ray[..., 256:259] * 2 - 1).reshape(B, Rh, Rw, 3).permute(0, 3, 1, 2).contiguous()
             depth = ray[..., 259:260].contiguous()
         ctx.tapes = (P, rtape, stape, cfg, passes, names)
-        ctx.mark_non_differentiable(depth)
-        return rgb, rgb_render, depth
+        ctx.mark_non_differentiable(depth, rec, z_vals)
+        return rgb, rgb_render, depth, rec, z_vals
 
     @staticmethod
     @torch.amp.custom_bwd(device_type="cuda")
     @torch.autograd.function.once_differentiable
-    def backward(ctx, d_rgb, d_rgb_render, d_depth):
+    def backward(ctx, d_rgb, d_rgb_render, d_depth, d_rec, d_z_vals):
         from . import synthesis_train
         if ctx.tapes is None:
             raise RuntimeError("hg3d: the generator's activation tape was released by a previous backward pass "

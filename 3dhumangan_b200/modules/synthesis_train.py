@@ -29,6 +29,12 @@ then the same dgrad / wgrad kernels run on `pre`, followed by
     hg_bilinear_adjoint    dP_lr (render resolution)
 and once, at the end, d(feature maps) = dP_lr . W_shared (wgmma `hg_linear`, K <= 256 per launch) and dW_shared = dP_lr^T . features
 (a plain library GEMM through torch.matmul).
+
+Eval mode (`training=False`: latent inversion, fine-tuning with frozen statistics) is the same schedule with less in it:
+the tables come from the running statistics and the stored spectral-norm u / v (no statistics epilogue, no power
+iteration, no buffer is written, no collective), so the statistics leaves and with them the a[c] + k[c]*x term do not
+exist.  A weight-gradient kernel is launched only for parameters that require grad; with every parameter frozen the
+backward is the data-gradient chain to the fixed style and the render features alone.
 """
 from __future__ import annotations
 
@@ -69,8 +75,9 @@ class SynthesisTape:
 
 
 def synthesis_forward_train(params, feat_lr, fixed_style, cfg, *, passes=3, prefix="synthesis_network.",
-                            input_prefix="synthesis_input.", process_group=None):
-    """-> (rgb [B,3,Hg,Wg] (no autograd history), tape).  `params`: name -> tensor (Parameters keep their .grad)."""
+                            input_prefix="synthesis_input.", process_group=None, training=True):
+    """-> (rgb [B,3,Hg,Wg] (no autograd history), tape).  `params`: name -> tensor (Parameters keep their .grad).
+    `training=False`: BatchNorm from the running statistics, spectral norm from the stored u / v; no buffer is written."""
     abi.require_device()
     P = params
     dev = fixed_style.device
@@ -82,7 +89,7 @@ def synthesis_forward_train(params, feat_lr, fixed_style, cfg, *, passes=3, pref
     T = (HW + 127) // 128
     nb = cfg["synthesis_blocks"]
     halves = [(k, j) for k in range(nb) for j in range(2)]
-    world = dist.get_world_size(process_group) if (dist.is_available() and dist.is_initialized()) else 1
+    world = dist.get_world_size(process_group) if (training and dist.is_available() and dist.is_initialized()) else 1
     f32 = dict(dtype=torch.float32, device=dev)
     blk = lambda k: f"{prefix}network.m3d_{k}."
     sp = lambda k, j: blk(k) + f"spade_{j}."
@@ -127,11 +134,11 @@ def synthesis_forward_train(params, feat_lr, fixed_style, cfg, *, passes=3, pref
     jc = torch.linspace(-1, 1, Wg, **f32)
     x0 = torch.empty(T, C, 128, **f32)
     w_in = P[input_prefix + "network.0.weight"].detach().reshape(C, 2).contiguous()
-    abi.synth_input(w_in, P[input_prefix + "network.0.bias"].detach(), ic, jc, x0, stats[0], B)
+    abi.synth_input(w_in, P[input_prefix + "network.0.bias"].detach(), ic, jc, x0, stats[0] if training else None, B)
     tape.input = dict(w=w_in, b=P[input_prefix + "network.0.bias"].detach(), ic=ic, jc=jc, prefix=input_prefix)
 
     # spectral normalisation of the 18 convolutions: one launch (power iteration, buffers in place), W / sigma with history
-    w_sns = sn_weights(P, [blk(k) + f"conv_{j}." for k, j in halves], True)
+    w_sns = sn_weights(P, [blk(k) + f"conv_{j}." for k, j in halves], training)
 
     rgb_cur = None
     cur, cur_bstride = x0, 0
@@ -142,11 +149,15 @@ def synthesis_forward_train(params, feat_lr, fixed_style, cfg, *, passes=3, pref
         if world > 1:
             all_reduce_stats(srow, process_group)
         count = float(B * HW * world)
-        # leaves of the batch statistics: their gradients are the a[c], k[c] of dL/dx
-        ssum = srow[:C].clone().requires_grad_(True)
-        ssq = srow[C:2 * C].clone().requires_grad_(True)
         pixel = (k, j) in pxi
-        mod = spade_table(P, bn, ssum, ssq, count, None if pixel else GB[(k, j)])
+        if training:
+            # leaves of the batch statistics: their gradients are the a[c], k[c] of dL/dx
+            ssum = srow[:C].clone().requires_grad_(True)
+            ssq = srow[C:2 * C].clone().requires_grad_(True)
+            mod = spade_table(P, bn, ssum, ssq, count, None if pixel else GB[(k, j)])
+        else:
+            ssum = ssq = None
+            mod = spade_table_eval(P, bn, None if pixel else GB[(k, j)])
         conv = blk(k) + f"conv_{j}."
         w_sn = w_sns[conv].reshape(C, C)
         wimg = abi.pack_weight(w_sn.detach().contiguous(), Nb=256)[0]
@@ -177,10 +188,10 @@ def synthesis_forward_train(params, feat_lr, fixed_style, cfg, *, passes=3, pref
             rec.update(i=i, spade=s_, p_bias=p_bias, p_bias_d=p_bias_d, wg=wg, wb=wb, bg1=(bg + 1.0).contiguous(), bb=bb)
             _spade(cur, cur_bstride, wimg, P[conv + "bias"].detach(), out, B, Hg, Wg, passes, scsh=mod_d,
                    p_lr=p_lr[:, i * 128:], p_stride=p_lr.shape[1], p_bias=p_bias_d, wgb=abi.pack_weight(w_il, Nb=256)[0],
-                   bgb=b_il, Rh=Rh, Rw=Rw, skip=block_in[0] if use_skip else None, stats=stats[idx + 1], **kw)
+                   bgb=b_il, Rh=Rh, Rw=Rw, skip=block_in[0] if use_skip else None, stats=stats[idx + 1] if training else None, **kw)
         else:
             _spade(cur, cur_bstride, wimg, P[conv + "bias"].detach(), out, B, Hg, Wg, passes, mod=mod_d,
-                   skip=block_in[0] if use_skip else None, stats=stats[idx + 1], **kw)
+                   skip=block_in[0] if use_skip else None, stats=stats[idx + 1] if training else None, **kw)
         if use_rgb:
             rgb_cur = rgb_next
         tape.halves.append(rec)
@@ -205,20 +216,28 @@ def spade_table(P, bn, ssum, ssq, count, gb=None):
     map3d_layers.py:162)."""
     mean = ssum / count
     var = (ssq / count - mean * mean).clamp_min(0.0)
-    rstd = torch.rsqrt(var + 1e-5)
-    sc = P[bn + "weight"].double() * rstd
-    sh = P[bn + "bias"].double() - mean * sc
-    if gb is None:      # BatchNorm scale/shift only; gamma/beta are per pixel
-        mod = torch.stack([sc, sh]).float()
-    else:
-        G, Bt = gb
-        mod = torch.stack([sc[None, :] * G.double(), sh[None, :] * G.double() + Bt.double()], dim=1).float()
+    mod = _fold(P, bn, mean, var, gb)
     with torch.no_grad():
         P[bn + "running_mean"].mul_(0.9).add_(0.1 * mean.float())
         P[bn + "running_var"].mul_(0.9).add_(0.1 * (var * count / max(count - 1, 1)).float())
         if (bn + "num_batches_tracked") in P:
             P[bn + "num_batches_tracked"] += 1
     return mod
+
+
+def spade_table_eval(P, bn, gb=None):
+    """`spade_table` in eval mode: the table from the running statistics, with autograd history from the BatchNorm weight /
+    bias (and gb) only; no buffer is written."""
+    return _fold(P, bn, P[bn + "running_mean"].detach().double(), P[bn + "running_var"].detach().double(), gb)
+
+
+def _fold(P, bn, mean, var, gb):
+    sc = P[bn + "weight"].double() * torch.rsqrt(var + 1e-5)
+    sh = P[bn + "bias"].double() - mean * sc
+    if gb is None:      # BatchNorm scale/shift only; gamma/beta are per pixel
+        return torch.stack([sc, sh]).float()
+    G, Bt = gb
+    return torch.stack([sc[None, :] * G.double(), sh[None, :] * G.double() + Bt.double()], dim=1).float()
 
 
 def grad_accumulator(P, grads):
@@ -268,6 +287,7 @@ def synthesis_backward(params, tape, drgb, *, passes=3, grads=None):
     full = T * HALF * 128
     new = lambda: torch.empty(B, T, HALF, 128, **f32)
     acc = grad_accumulator(P, grads)
+    need = lambda *names: any(P[k].requires_grad for k in names)      # a weight-gradient kernel runs only for these
 
     def conv_wgrad(d, xs, x_bstride, mods_in):
         """[nh*256, nh*256] weight gradient of a half-block's convolution block by block, [nh*256] bias gradient."""
@@ -296,19 +316,22 @@ def synthesis_backward(params, tape, drgb, *, passes=3, grads=None):
         for c in halves:
             ckw = {}
             if rec["rgb"] is not None:
-                dwrgb.append(torch.zeros(3, HALF, dtype=torch.float64, device=dev))
+                dwrgb.append(torch.zeros(3, HALF, dtype=torch.float64, device=dev) if need(rec["rgb"] + "weight") else None)
                 ckw = dict(drgb=drgb, rgb_w=rec["rgb_w"][:, sl(c)].contiguous(), dwrgb=dwrgb[c])
             if nxt is not None:
                 ckw.update(dpre=nxt[0][c], g1=nxt[1][c], ak=nxt[2][c])
             d.append(abi.spade_bwd_combine(new(), B=B, Hg=Hg, Wg=Wg, x=rec["out"][c], x_bstride=full, dskip=dskip[c], **ckw))
         if rec["rgb"] is not None:
-            acc(rec["rgb"] + "weight", torch.cat(dwrgb, -1)[:, :C].float())
+            if dwrgb[0] is not None:
+                acc(rec["rgb"] + "weight", torch.cat(dwrgb, -1)[:, :C].float())
             acc(rec["rgb"] + "bias", drgb_sum)
         dout[h] = d
         dout.pop(h + 3, None)
         # ---- this half-block: const style acts on x through its table, pixel style on the rebuilt `pre`
         Wsn = _pad2(rec["w_sn"].detach().reshape(C, C), W2, W2)
         sums = [torch.zeros(B, 2, HALF, dtype=torch.float64, device=dev) for _ in halves]
+        want_w = need(rec["conv"] + "weight_orig", rec["conv"] + "bias")
+        dW = db = None
         if rec["pixel"]:
             Rh, Rw = cfg["render_height"], cfg["render_width"]
             i = rec["i"]
@@ -329,7 +352,8 @@ def synthesis_backward(params, tape, drgb, *, passes=3, grads=None):
             # conv data / weight gradients on pre (y = lrelu(pre))
             dpre = [abi.conv1x1_blocked_bwd(d[0], pre[c], _packT(Wsn, c), new(), sums[c], g2=d[1] if nh == 2 else None, **kw)
                     for c in halves]
-            dW, db = conv_wgrad(d, pre, full, (None,) * nh)
+            if want_w:
+                dW, db = conv_wgrad(d, pre, full, (None,) * nh)
             # modulation: dxn (over pre), dgam (over gam), BatchNorm scale/shift sums
             s3 = [torch.zeros(3, HALF, dtype=torch.float64, device=dev) for _ in halves]
             for c in halves:
@@ -348,6 +372,8 @@ def synthesis_backward(params, tape, drgb, *, passes=3, grads=None):
                 da1 = part if da1 is None else da1.add_(part)
             sp_ = rec["spade"]
             for gs, nm in ((dgam, "mlp_gamma."), (dpre, "mlp_beta.")):
+                if not need(sp_ + nm + "weight", sp_ + nm + "bias"):
+                    continue
                 dws, dbs = zip(*[abi.spade_bwd_wgrad(gs[c], a1, T * 128 * 128, None, Cx=128, **kw) for c in halves])
                 acc(sp_ + nm + "weight", torch.cat(dws)[:C])
                 acc(sp_ + nm + "bias", torch.cat(dbs)[:C])
@@ -369,39 +395,46 @@ def synthesis_backward(params, tape, drgb, *, passes=3, grads=None):
             else:
                 dpre = [abi.conv1x1_blocked_bwd(d[0], rec["x"][c], _packT(Wsn, c), new(), sums[c], g2=d[1], mod=rec["mod_d"][c],
                                                 slope=0.2, **kw) for c in halves]
-            dW, db = conv_wgrad(d, rec["x"], rec["x_bstride"], rec["mod_d"])
+            if want_w:
+                dW, db = conv_wgrad(d, rec["x"], rec["x_bstride"], rec["mod_d"])
             # d g1 = sum dpre*x, d g0 = sum dpre
             dmod = torch.stack([torch.cat([s[:, 1] for s in sums], -1), torch.cat([s[:, 0] for s in sums], -1)], dim=1).float()
             g1_tab = rec["mod_d"]
-        acc(rec["conv"] + "bias", db[:C])
-        small_out.append(rec["w_sn"])
-        small_grad.append(dW[:C, :C].reshape(rec["w_sn"].shape))
-        ga, gk = torch.autograd.grad(rec["mod"], [rec["ssum"], rec["ssq"]], grad_outputs=dmod, retain_graph=True)
-        ak = torch.stack([ga, gk])
-        if tape.world > 1:          # SyncBatchNorm: every rank's loss depends on the global statistics
-            dist.all_reduce(ak, group=tape.process_group)
-        ak = torch.stack([ak[0], 2.0 * ak[1]]).float()                     # d(sum x)/dx = 1, d(sum x^2)/dx = 2x
+        if want_w:
+            acc(rec["conv"] + "bias", db[:C])
+            small_out.append(rec["w_sn"])
+            small_grad.append(dW[:C, :C].reshape(rec["w_sn"].shape))
+        if rec["ssum"] is None:     # eval mode: the statistics are constants, dL/dx has no a + k*x term
+            aks = (None,) * nh
+        else:
+            ga, gk = torch.autograd.grad(rec["mod"], [rec["ssum"], rec["ssq"]], grad_outputs=dmod, retain_graph=True)
+            ak = torch.stack([ga, gk])
+            if tape.world > 1:          # SyncBatchNorm: every rank's loss depends on the global statistics
+                dist.all_reduce(ak, group=tape.process_group)
+            ak = torch.stack([ak[0], 2.0 * ak[1]]).float()                     # d(sum x)/dx = 1, d(sum x^2)/dx = 2x
+            aks = [ak[:, sl(c)].contiguous() for c in halves]
         small_out.append(rec["mod"])
         small_grad.append(dmod)
-        nxt = (dpre, g1_tab, [ak[:, sl(c)].contiguous() for c in halves])
+        nxt = (dpre, g1_tab, aks)
     # ---- gradient w.r.t. the synthesis input, then its two parameters, per half
     ip = tape.input["prefix"]
     dw_in, db_in = [], []
-    for c in halves:
+    for c in halves if need(ip + "network.0.weight", ip + "network.0.bias") else ():
         dx0 = abi.spade_bwd_combine(new(), B=B, Hg=Hg, Wg=Wg, x=H[0]["x"][c], x_bstride=H[0]["x_bstride"], dpre=nxt[0][c], g1=nxt[1][c],
                                     ak=nxt[2][c])
         dw, db = abi.synth_input_bwd(dx0, tape.input["w"][sl(c)].contiguous(), tape.input["b"][sl(c)].contiguous(),
                                      tape.input["ic"], tape.input["jc"], B)
         dw_in.append(dw)
         db_in.append(db)
-    acc(ip + "network.0.weight", torch.cat(dw_in)[:C])
-    acc(ip + "network.0.bias", torch.cat(db_in)[:C])
+    if dw_in:
+        acc(ip + "network.0.weight", torch.cat(dw_in)[:C])
+        acc(ip + "network.0.bias", torch.cat(db_in)[:C])
     # ---- all [C]- and [B,C]-sized chains in one autograd pass
     fs = tape.fixed_style
     leaves = [t for t in small_out if t.requires_grad]
     small = [g for t, g in zip(small_out, small_grad) if t.requires_grad]
     names = [k for k, p in P.items() if isinstance(p, torch.Tensor) and p.requires_grad and p.is_leaf]
-    res = torch.autograd.grad(leaves, [P[k] for k in names] + [fs], small, allow_unused=True)
+    res = torch.autograd.grad(leaves, [P[k] for k in names] + [fs], small, allow_unused=True) if leaves else [None]
     for k, r in zip(names, res[:-1]):
         if r is not None:
             acc(k, r)
@@ -411,11 +444,12 @@ def synthesis_backward(params, tape, drgb, *, passes=3, grads=None):
     if tape.px and "dp" in tape.p:
         dp, Ws, X = tape.p["dp"], tape.p["Ws"], tape.p["X"]
         dfeat = _gemm_nt(dp, Ws.t().contiguous(), passes=passes).reshape(B, -1, C)
-        prev = torch.backends.cuda.matmul.allow_tf32
-        torch.backends.cuda.matmul.allow_tf32 = False
-        dWs = dp.t() @ X                                                             # [n*128, C]  (plain library GEMM)
-        torch.backends.cuda.matmul.allow_tf32 = prev
-        for rec in H:
-            if rec["pixel"]:
-                acc(rec["spade"] + "mlp_shared.0.weight", dWs[rec["i"] * 128:(rec["i"] + 1) * 128])
+        shared = [rec for rec in H if rec["pixel"] and need(rec["spade"] + "mlp_shared.0.weight")]
+        if shared:
+            prev = torch.backends.cuda.matmul.allow_tf32
+            torch.backends.cuda.matmul.allow_tf32 = False
+            dWs = dp.t() @ X                                                             # [n*128, C]  (plain library GEMM)
+            torch.backends.cuda.matmul.allow_tf32 = prev
+        for rec in shared:
+            acc(rec["spade"] + "mlp_shared.0.weight", dWs[rec["i"] * 128:(rec["i"] + 1) * 128])
     return dfs, dfeat

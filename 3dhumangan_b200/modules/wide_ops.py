@@ -15,7 +15,8 @@ affine and zero FiLM tables, so they stay zero through every layer.
              gamma / beta by `hg_conv1x1_blocked`, pre = BN(x) * gamma + beta (`hg_spade_pixel_pre`), then the wide conv with
              an identity table -- the decomposition the 256-channel BACKWARD already uses.
 
-Inference and train-mode forward (batch statistics, running-stat and spectral-norm buffer updates).  Given a `tape`,
+Inference and train-mode forward (batch statistics, running-stat and spectral-norm buffer updates).  Given a `tape`
+(train mode, or eval mode with the running statistics and the stored spectral-norm u / v as constants),
 each forward also keeps what the backward of every width needs (render_train.mlp_backward,
 synthesis_train.synthesis_backward, over two 256-channel halves here), and builds the small tables that carry
 parameter gradients (FiLM, SPADE / BatchNorm, W / sigma) with autograd history.  Mirrors Map3DGenerator.render / forward (map3d_generator.py:208-280, 381-523),
@@ -83,13 +84,14 @@ def wide_layer(xs, W512, b512, *, mods=None, act=0, slope=0.2, skips=None, stats
 # ----------------------------------------------------------------------------------------------------------------------
 @torch.no_grad()
 def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix="neural_field.", tape=None, records=None,
-                        sigma_only=False):
+                        sigma_only=False, training=True):
     """-> ray features [B,R,C], rgb [B,R,3] (in [0,1], before the *2-1), depth [B,R,1].
     `tape` (a dict) receives what `render_train.mlp_backward` needs, in the format its docstring describes: per half the
     linear outputs lin_a, lin_b, out_0..3, lin_c, feat, then sig, rgbp and the FiLM tables built from freq / phase
     leaves with autograd history.
     `records` (rec [B,N,36], z_vals [B,N]) replaces the ray stage (hierarchical_sample: the merged samples, with
-    cfg["num_steps"] the samples per ray).  `sigma_only` stops after the sigma head and returns the raw sigma [B,N]."""
+    cfg["num_steps"] the samples per ray).  `sigma_only` stops after the sigma head and returns the raw sigma [B,N].
+    `training` matters with a tape only: `last_back=True` is differentiated for an eval-mode module, refused in train mode."""
     from . import render_train
     abi.require_device()
     g = lambda n: P[prefix + n].detach().float()
@@ -99,7 +101,7 @@ def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix
         raise RuntimeError("hg3d: the zero-padded path serves hidden_dim <= 512")
     if cfg.get("neural_field_blocks", 4) != 4:
         raise RuntimeError("hg3d: the renderer is built for neural_field_blocks == 4 (all shipped curricula)")
-    if tape is not None and cfg.get("last_back", False):
+    if tape is not None and training and cfg.get("last_back", False):
         raise RuntimeError("hg3d: last_back=True is an inference-only setting (eval_last_back); the training renderer does not build it")
     if records is None and cfg.get("hierarchical_sample", False):
         from . import hierarchical
@@ -193,7 +195,6 @@ def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix
     if taped:
         with torch.enable_grad():      # colour bias and direction columns, with history (cf. render_train.mlp_forward_train)
             bcol_t = P[prefix + "color_layer_sine.layer.bias"] + P[prefix + "color_layer_sine.layer.weight"][:, :3] @ dvec
-        del comp["last_back"]
         tape.update(P=P, prefix=prefix, C=C, Fd=Fd, B=B, N=N, R=R, geo_dim=geo_dim, kw=kw, fq=fq, ph=ph, mods_h=mods_h, mods=mods,
                     outs=outs + [out3], lin_c=lin_c, feat=feat, sig=sig, rgbp=rgbp, z=z_vals, noise=nz, comp=comp, bcol=bcol_t,
                     w_sigma=w_sigma, w_rgb=w_rgb)
@@ -208,9 +209,10 @@ def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix
 def synthesis_forward_wide(P, feats, fixed_style, cfg, *, training=True, passes=3, prefix="synthesis_network.",
                            input_prefix="synthesis_input.", process_group=None, tape=None):
     """feats [B, Rh*Rw, C] render-resolution features, fixed_style [B,C] -> rgb [B,3,Hg,Wg].
-    `tape` (a `synthesis_train.SynthesisTape`, training only) receives what `synthesis_train.synthesis_backward` needs:
+    `tape` (a `synthesis_train.SynthesisTape`) receives what `synthesis_train.synthesis_backward` needs:
     per half-block its input halves, the SPADE tables built with autograd from sum(x) / sum(x^2) leaves (instead of
-    hg_bn_finalize), W / sigma with history and the skip / ToRGB bookkeeping, in the format of that class."""
+    hg_bn_finalize), W / sigma with history and the skip / ToRGB bookkeeping, in the format of that class.  With
+    `training=False` the taped tables come from the running statistics (no leaves) and no buffer is written."""
     abi.require_device()
     dev = feats.device
     B = feats.shape[0]
@@ -222,7 +224,7 @@ def synthesis_forward_wide(P, feats, fixed_style, cfg, *, training=True, passes=
     T = (HW + 127) // 128
     nb = cfg["synthesis_blocks"]
     mode = cfg.get("map3d_mode", "isolated")
-    world = dist.get_world_size(process_group) if (dist.is_available() and dist.is_initialized()) else 1
+    world = dist.get_world_size(process_group) if (training and dist.is_available() and dist.is_initialized()) else 1
     f32 = dict(dtype=torch.float32, device=dev)
     halves = [(k, j) for k in range(nb) for j in range(2)]
     blk = lambda k: f"{prefix}network.m3d_{k}."
@@ -236,10 +238,8 @@ def synthesis_forward_wide(P, feats, fixed_style, cfg, *, training=True, passes=
     pxi = {key: i for i, key in enumerate(px)}
     taped = tape is not None
     if taped:
-        if not training:
-            raise RuntimeError("hg3d: gradients through the generator are built for train() mode (batch statistics)")
         with torch.enable_grad():
-            w_sns = sn_weights(P, conv_names, True)
+            w_sns = sn_weights(P, conv_names, training)
         fs = fs.detach().requires_grad_(True)           # leaf: its gradient is returned by the backward
         tape.cfg, tape.B, tape.fixed_style, tape.px = cfg, B, fs, px
         tape.process_group, tape.world = process_group, world
@@ -291,7 +291,8 @@ def synthesis_forward_wide(P, feats, fixed_style, cfg, *, training=True, passes=
             for h in (0, 1):
                 all_reduce_stats(stats[idx, h], process_group)
         if taped:
-            mod, tables, ssum, ssq = _taped_tables(P, stats[idx], bn, sp(k, j), fs, pixel, C, float(B * HW * world))
+            mod, tables, ssum, ssq = _taped_tables(P, stats[idx] if training else None, bn, sp(k, j), fs, pixel, C,
+                                                   float(B * HW * world))
         else:
             tables = _tables(P, stats[idx], bn, sp(k, j), fs, pixel, C, B, training, passes)
         if j == 0:
@@ -352,14 +353,18 @@ def synthesis_forward_wide(P, feats, fixed_style, cfg, *, training=True, passes=
 
 
 def _taped_tables(P, srow, bn, s, fs, pixel, C, count):
-    """Training forward with a tape: the SPADE table of one half-block by `synthesis_train.spade_table` from the leaves
-    sum(x), sum(x^2) [512] of its batch statistics (both halves), zero-padded to 512 channels.
+    """Forward with a tape: the SPADE table of one half-block by `synthesis_train.spade_table` from the leaves
+    sum(x), sum(x^2) [512] of its batch statistics (both halves), zero-padded to 512 channels; srow None (eval mode):
+    by `spade_table_eval` from the running statistics, without leaves.
     -> (table [(B,)2,512] with history, its two detached halves, ssum, ssq)."""
-    from .synthesis_train import const_gamma_beta, spade_table
-    ssum = srow[:, :HALF].reshape(2 * HALF).clone().requires_grad_(True)
-    ssq = srow[:, HALF:2 * HALF].reshape(2 * HALF).clone().requires_grad_(True)
+    from .synthesis_train import const_gamma_beta, spade_table, spade_table_eval
+    ssum = ssq = None
+    if srow is not None:
+        ssum = srow[:, :HALF].reshape(2 * HALF).clone().requires_grad_(True)
+        ssq = srow[:, HALF:2 * HALF].reshape(2 * HALF).clone().requires_grad_(True)
     with torch.enable_grad():
-        mod = spade_table(P, bn, ssum[:C], ssq[:C], count, None if pixel else const_gamma_beta(P, s, fs, C))
+        gb = None if pixel else const_gamma_beta(P, s, fs, C)
+        mod = spade_table(P, bn, ssum[:C], ssq[:C], count, gb) if srow is not None else spade_table_eval(P, bn, gb)
         mod = F.pad(mod, (0, 2 * HALF - C))          # padded channels: g1 = g0 = 0
     return mod, [mod[..., :HALF].detach().contiguous(), mod[..., HALF:].detach().contiguous()], ssum, ssq
 

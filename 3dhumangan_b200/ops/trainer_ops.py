@@ -2,6 +2,8 @@
 
   seg_ce_balanced   PhaseTrainer._calculate_segmentation_loss, mode 'cross_entropy_balanced' (phase_trainer.py:203-256):
                     label histogram -> per-class coefficients -> ONE pass over the logits that yields the loss and its gradient.
+  image_loss        reconstruction loss of latent inversion (inversion.py): weighted L2 or Charbonnier over an image, value
+                    and gradient in one pass.
   FusedAdam         torch.optim.Adam (same state_dict: step / exp_avg / exp_avg_sq, same arithmetic) for the reference's
                     parameter groups (phase_trainer.py:57-76) with global-norm clipping (clip_grad_norm_, :314,336) and the
                     generator's EMA (lib/components/ema.py:29-48) folded into the same multi-tensor launch.
@@ -63,6 +65,52 @@ def seg_ce_balanced(segments, gt, label_dim, prior_weights=None):
     if prior_weights is not None:
         prior = torch.as_tensor(prior_weights, dtype=torch.float32, device=segments.device).contiguous()
     return _SegCE.apply(segments, gt, prior, int(label_dim))
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# image reconstruction loss
+# ----------------------------------------------------------------------------------------------------------------------
+class _ImageLoss(torch.autograd.Function):
+    @staticmethod
+    @torch.amp.custom_fwd(device_type="cuda", cast_inputs=torch.float32)
+    def forward(ctx, pred, target, mask, mode, eps):
+        abi.require_device()
+        B = pred.shape[0]
+        if pred.dim() != 4 or pred.shape[1] != 3 or target.shape != pred.shape:
+            raise RuntimeError("hg3d: image_loss expects prediction and target [B,3,H,W] of one shape")
+        HW = pred.shape[2] * pred.shape[3]
+        if mask is not None and mask.numel() != B * HW:
+            raise RuntimeError("hg3d: image_loss expects a weight mask [B,1,H,W]")
+        pred, target = pred.contiguous(), target.contiguous()
+        mask = None if mask is None else mask.contiguous()
+        dev = pred.device
+        loss = torch.empty(1, dtype=torch.float32, device=dev)
+        ws = torch.empty(2 * torch.cuda.get_device_properties(dev).multi_processor_count, dtype=torch.float64, device=dev)
+        dpred = torch.empty_like(pred) if ctx.needs_input_grad[0] else None
+        with torch.cuda.device_of(pred):
+            abi.call("hg_image_loss", abi.ptr(pred), abi.ptr(target), abi.ptr(mask), abi.ptr(dpred), abi.ptr(loss), abi.ptr(ws), B, HW,
+                     mode, float(eps), abi.stream())
+        ctx.save_for_backward(dpred)
+        return loss.reshape(())
+
+    @staticmethod
+    @torch.amp.custom_bwd(device_type="cuda")
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g):
+        (dpred,) = ctx.saved_tensors
+        return (dpred * g if dpred is not None else None), None, None, None, None
+
+
+def image_loss(pred, target, mask=None, kind="l2", eps=1e-3):
+    """mean over the B*3*H*W elements of mask * rho(pred - target): rho(d) = d^2 (`kind="l2"`) or the Charbonnier
+    sqrt(d^2 + eps^2) (`kind="charbonnier"`, a smooth L1).  `mask` [B,1,H,W] fp32 weights each pixel (the person's
+    silhouette: `preprocess.Preprocessor` labels != background) or None.  Differentiable w.r.t. `pred` (first order); the
+    value repeats bit for bit (fp64 partial sums in a fixed order)."""
+    if kind not in ("l2", "charbonnier"):
+        raise RuntimeError(f"hg3d: image_loss kind {kind!r} is not built ('l2' or 'charbonnier')")
+    if mask is not None:
+        mask = mask.to(torch.float32)
+    return _ImageLoss.apply(pred, target, mask, 0 if kind == "l2" else 1, eps)
 
 
 # ----------------------------------------------------------------------------------------------------------------------

@@ -200,17 +200,18 @@ int hg_act_wgrad_blocked(const float* dout, const float* pscale, const float* x,
  *                       (mod3 [B,2,256] = f, phi of the last FiLM slice; modulated.py:62-73).
  * hg_render_heads_bwd:  acc[4*256+4] fp64 += (d w_sigma, d W_rgb[0..2], d b[0..3]).
  * hg_render_composite(_bwd): vr.ray_integration (volume_rendering.py:12-56) and its gradient; ray_out / dray [B,R,260] =
- *                       feat(256) | rgb(3) | depth; last_back in the forward only; S in {8,16,32,64,128}. */
+ *                       feat(256) | rgb(3) | depth; last_back: the last sample of a ray absorbs 1 - sum w before the sums
+ *                       (eval_last_back of the sample app), in the forward and its gradient; S in {8,16,32,64,128}. */
 int hg_render_heads(const float* out3, const float* linc, const float* mod3, const float* w_sigma, const float* w_rgb,
                     const float* heads_b, float* sig, float* rgbp, int B, int N, void* stream);
 int hg_render_heads_bwd(const float* out3, const float* linc, const float* mod3, const float* dsig, const float* drgbp,
                         double* acc, int B, int N, void* stream);
 int hg_render_composite(const float* sig, const float* z, const float* noise, const float* rgbp, const float* feat,
                         float* ray_out, float* weights, int B, int R, int S, float noise_std, int white_back,
-                        int clamp_softplus, int last_back /* forward only: eval_last_back of the sample app */, void* stream);
+                        int clamp_softplus, int last_back, void* stream);
 int hg_render_composite_bwd(const float* sig, const float* z, const float* noise, const float* rgbp, const float* feat,
                             const float* dray, float* dfeat, float* drgbp, float* dsig, int B, int R, int S,
-                            float noise_std, int white_back, int clamp_softplus, void* stream);
+                            float noise_std, int white_back, int clamp_softplus, int last_back, void* stream);
 int hg_wgrad_blocked(const float* dout, const float* x, long x_bstride, int Cx, const float* mod, float* dw, float* dbias,
                      void* workspace, int B, int C, int Hg, int Wg, int passes, void* stream);
 int hg_spade_a1(const float* p_lr, long p_stride, const float* p_bias, float* a1, int B, int Hg, int Wg, int Rh, int Rw,
@@ -321,6 +322,11 @@ int hg_label_histogram(const long* labels, long n, int L, int* hist, void* strea
 int hg_seg_ce_coef(const int* hist, const float* prior /* [L] or NULL */, int L, double numel, float* coef, void* stream);
 int hg_seg_ce(const float* logits, const long* labels, const float* coef, float* dlogits /* or NULL */, float* loss,
               double* workspace /* >= 2 * #SMs doubles */, int B, int L, long HW, void* stream);
+/* Image reconstruction loss of latent inversion: loss[0] = mean over the B*3*HW elements of mask[b,p] * rho(pred - target),
+ * rho(d) = d^2 (mode 0) or the Charbonnier sqrt(d^2 + eps^2) (mode 1), and optionally d loss / d pred, in one pass; fp64
+ * block partials summed in a fixed order.  pred / target [B,3,HW], mask [B,HW] or NULL (all ones). */
+int hg_image_loss(const float* pred, const float* target, const float* mask, float* dpred /* or NULL */, float* loss,
+                  double* workspace /* >= 2 * #SMs doubles */, int B, long HW, int mode, float eps, void* stream);
 /* Multi-tensor global-norm clipping (torch.nn.utils.clip_grad_norm_, phase_trainer.py:314,336), torch.optim.Adam's update
  * with per-group scalars (phase_trainer.py:57-76) and the generator's EMA (lib/components/ema.py:29-48) over a device table
  * of tensors: entries { float* p, g, exp_avg, exp_avg_sq, ema; long n } (hg_mt_entry_bytes() = 48; g NULL = no gradient this
