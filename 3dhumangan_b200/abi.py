@@ -79,6 +79,11 @@ SIGNATURES = {
     "hg_seg_ce_coef": (c_int, [c_void_p, c_void_p, c_int, c_double, c_void_p, c_void_p]),
     "hg_seg_ce": (c_int, [c_void_p] * 6 + [c_int, c_int, c_long, c_void_p]),
     "hg_image_loss": (c_int, [c_void_p] * 6 + [c_int, c_long, c_int, c_float, c_void_p]),
+    "hg_vgg_input": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
+    "hg_vgg_input_adjoint": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
+    "hg_maxpool2x2": (c_int, [c_void_p, c_void_p, c_long, c_int, c_int, c_void_p]),
+    "hg_vgg_level_bwd": (c_int, [c_void_p] * 4 + [c_float, c_void_p, c_long, c_int, c_int, c_void_p]),
+    "hg_smooth_l1": (c_int, [c_void_p, c_void_p, c_long, c_void_p, c_void_p, c_void_p]),
     "hg_mt_entry_bytes": (c_int, []),
     "hg_mt_chunk_bytes": (c_int, []),
     "hg_mt_chunk_elems": (c_int, []),

@@ -9,6 +9,12 @@ jitter is drawn once: the point records of the first render (ray samples, neares
 by every later step, so every step differentiates one fixed function; a given seed repeats the run up to the order of the
 atomic sums in the data-gradient kernels (the last bits of a gradient).
 With `hierarchical_sample=True` the fine samples follow the density and every step redraws them from a per-step seed.
+
+`perceptual` (a `perceptual.VGGPerceptualLoss`) adds the reference trainer's feature-space term (phase_trainer.py:515-520):
+sum_i perceptual_lambda[i] * L_i(0.5 * rgbs + 0.5, 0.5 * target + 0.5), the target's VGG features computed once before the
+loop.  `loss=None` drops the pixel term.  A merged training config passed through **kwargs carries its own `perceptual_lambda`
+(zeros in every shipped configuration), which then takes this argument's place; all-zero weights with a `perceptual`
+module raise rather than silently drop the term.
 """
 from __future__ import annotations
 
@@ -18,14 +24,22 @@ from . import abi
 from .ops.trainer_ops import FusedAdam, image_loss
 
 
-def invert(G, target, conditions, *, space="film", steps=100, lr=0.01, mask=None, seed=0, loss="l2", **kwargs):
+def invert(G, target, conditions, *, space="film", steps=100, lr=0.01, mask=None, seed=0, loss="l2", perceptual=None,
+           perceptual_lambda=(1, 1, 1, 1), **kwargs):
     """target [B,3,gen_height,gen_width] in [-1,1]; conditions: the SMPL / camera dict of `Map3DGenerator.forward`;
     kwargs: the merged config that `forward` takes (render_height, render_width, num_steps, last_back, ...).
     -> dict(variables={name: tensor}, losses=[float per step], image=[B,3,H,W] of the optimised variables).
     Without hierarchical_sample `losses` and `image` are values of one function (the jitter of the first render).  With it
-    every step and the final image draw their own samples (seed + step), so the curve is that of a stochastic objective."""
+    every step and the final image draw their own samples (seed + step), so the curve is that of a stochastic objective.
+    The objective is image_loss(kind=loss) (`mask` weights this pixel term only; `loss=None` drops it) plus, with
+    `perceptual`, the perceptual term above."""
     if space not in ("z", "film"):
         raise RuntimeError(f"hg3d: inversion space {space!r} is not built ('z' or 'film')")
+    if loss is None and perceptual is None:
+        raise RuntimeError("hg3d: inversion needs a pixel loss, a perceptual loss or both")
+    if perceptual is not None and not any(float(w) for w in perceptual_lambda):
+        raise RuntimeError(f"hg3d: perceptual_lambda {list(perceptual_lambda)} switches the perceptual term off; pass non-zero "
+                           "weights (a merged config's own perceptual_lambda overrides the default)")
     abi.require_device()
     dev = target.device
     B = target.shape[0]
@@ -37,6 +51,9 @@ def invert(G, target, conditions, *, space="film", steps=100, lr=0.01, mask=None
     for p, _ in frozen:
         p.requires_grad_(False)
     try:
+        target_features = None
+        if perceptual is not None:
+            target_features = perceptual.target_features(0.5 * target + 0.5)
         z = torch.randn(B, G.latent_dim, generator=torch.Generator(device=dev).manual_seed(seed), device=dev)
         if space == "z":
             variables = {"z": z.requires_grad_(True)}
@@ -68,7 +85,9 @@ def invert(G, target, conditions, *, space="film", steps=100, lr=0.01, mask=None
                         break
                     if not hier:
                         records = out["hg_records"]
-                    value = image_loss(out["rgbs"], target, mask, kind=loss)
+                    value = 0.0 if loss is None else image_loss(out["rgbs"], target, mask, kind=loss)
+                    if perceptual is not None:
+                        value = value + perceptual.loss(0.5 * out["rgbs"] + 0.5, target_features, perceptual_lambda)
                 for v in variables.values():
                     v.grad = None
                 value.backward()

@@ -341,6 +341,26 @@ int hg_mt_grad_norm(const void* table, const void* chunks, int nchunks, float ma
 int hg_mt_adam(const void* table, const void* chunks, int nchunks, const float* norm_clip /* or NULL */, const float* scalars,
                int ngroups, float ema_one_minus_decay, int write_clipped_grad, void* stream);
 
+/* ---- VGG16 perceptual loss (lib/components/perceptual_loss.py) around the hg_conv2d / hg_bias_act layers -------------------
+ * hg_vgg_input        : out [B,3,Ho,Wo] = bilinear resize (align_corners=False, no antialias) of (x - mean) / std, x [B,C,H,W]
+ *                       with C = 1 (repeated to 3 channels) or 3; mean / std [3] on the device; Ho x Wo == H x W: no resize.
+ * hg_vgg_input_adjoint: dx [B,C,H,W] = the transpose of hg_vgg_input's linear part applied to dout [B,3,Ho,Wo], as a gather
+ *                       (no atomics: repeats bit for bit).
+ * hg_maxpool2x2       : y [planes,H/2,W/2] = MaxPool2d(2, 2) of x [planes,H,W], floor semantics.
+ * hg_vgg_level_bwd    : dpre [planes,H,W] = [y > 0] * (unpool(dpool) + gscale[0] * inv_n * clamp(y - t, -1, 1)): the gradient at
+ *                       the last pre-activation of a block whose output y is compared with the target's t and then max-pooled;
+ *                       each window's gradient goes to its first maximum in row-major order.  dpool [planes,H/2,W/2] NULL: no
+ *                       pooled level follows; t and gscale (a device scalar) NULL together: no loss term.
+ * hg_smooth_l1        : loss[0] = mean over n elements of smooth_l1(a - b) with beta = 1; fp64 block partials summed in a fixed
+ *                       order. */
+int hg_vgg_input(const float* x, int C, int B, int H, int W, const float* mean, const float* std, float* out, int Ho, int Wo,
+                 void* stream);
+int hg_vgg_input_adjoint(const float* dout, int B, int Ho, int Wo, const float* std, float* dx, int C, int H, int W, void* stream);
+int hg_maxpool2x2(const float* x, float* y, long planes, int H, int W, void* stream);
+int hg_vgg_level_bwd(const float* y, const float* t, const float* dpool, const float* gscale, float inv_n, float* dpre, long planes,
+                     int H, int W, void* stream);
+int hg_smooth_l1(const float* a, const float* b, long n, float* loss, double* workspace /* >= 2 * #SMs doubles */, void* stream);
+
 /* ---- StyleGAN3 native ops named by the reference ---------------------------------------------- */
 /* y = clamp(act(x + b[(i / stepB) % sizeB]) * gain)   replaces bias_act.cpp:32 / bias_act.cu:24 (forward).
  * act: 1 linear 2 relu 3 lrelu 4 tanh 5 sigmoid 6 elu 7 selu 8 softplus 9 swish; clamp < 0 disables. */

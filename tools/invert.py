@@ -2,8 +2,10 @@
 eval-mode generator, then recover it from another seed with `3dhumangan_b200.inversion.invert` and print the loss curve.
     python tools/invert.py [--config 420|tiny] [--space film|z] [--steps 100] [--lr 0.02] [--loss l2|charbonnier]
                            [--hierarchical] [--checkpoint generator.pth]
+                           [--perceptual-weights vgg16-397923af.pth] [--perceptual-lambda 1 1 1 1] [--no-pixel-loss]
 Without --checkpoint the generator is randomly initialised and its running statistics come from three train-mode forwards
-(at random initialisation the eval-mode output overflows)."""
+(at random initialisation the eval-mode output overflows).  --perceptual-weights adds the VGG16 perceptual term
+(3dhumangan_b200.perceptual) with torchvision's VGG16 weight file; --perceptual-lambda weights its four blocks."""
 import argparse
 import copy
 import importlib
@@ -54,6 +56,9 @@ def main():
     ap.add_argument("--hierarchical", action="store_true")
     ap.add_argument("--checkpoint")
     ap.add_argument("--seed", type=int, default=5)
+    ap.add_argument("--perceptual-weights", metavar="PATH", help="torchvision's vgg16-397923af.pth: add the perceptual term")
+    ap.add_argument("--perceptual-lambda", type=float, nargs=4, default=[1.0, 1.0, 1.0, 1.0])
+    ap.add_argument("--no-pixel-loss", action="store_true", help="with --perceptual-weights: the perceptual term alone")
     args = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("invert: needs a CUDA device")
@@ -64,7 +69,14 @@ def main():
     torch.manual_seed(11)
     with torch.no_grad():
         target = G(torch.randn(1, cfg["latent_dim"], device="cuda"), cond, **cfg)["rgbs"]
-    res = inv.invert(G, target, cond, space=args.space, steps=args.steps, lr=args.lr, seed=args.seed, loss=args.loss, **cfg)
+    perceptual = None
+    if args.perceptual_weights:
+        perceptual = importlib.import_module("3dhumangan_b200.perceptual").VGGPerceptualLoss(weights=args.perceptual_weights).cuda()
+    elif args.no_pixel_loss:
+        raise SystemExit("invert: --no-pixel-loss needs --perceptual-weights")
+    res = inv.invert(G, target, cond, space=args.space, steps=args.steps, lr=args.lr, seed=args.seed,
+                     loss=None if args.no_pixel_loss else args.loss, perceptual=perceptual,
+                     **dict(cfg, perceptual_lambda=args.perceptual_lambda))
     every = max(1, args.steps // 10)
     print(json.dumps({"space": args.space, "steps": args.steps, "loss_first": res["losses"][0], "loss_last": res["losses"][-1],
                       "curve": res["losses"][::every],
