@@ -470,13 +470,20 @@ __global__ void __launch_bounds__(256) pixel_pre_kernel(const float* __restrict_
   }
 }
 
+// components n.. of v set to zero
+__device__ __forceinline__ float4 keep_first(float4 v, int n) {
+  return make_float4(n > 0 ? v.x : 0.f, n > 1 ? v.y : 0.f, n > 2 ? v.z : 0.f, 0.f);
+}
+
 // dxn = dpre*gam (over `pre_dxn`), dgam = dpre*(x*sc+sh) (over `gam_dgam`); per-channel sums
-//   sums[0][c] = sum dxn*x, sums[1][c] = sum dxn, sums[2][c] = sum dgam     (fp64, accumulated)
-// Same mapping as the combine kernel: warp w owns channels w, w+8, ..., a lane owns 4 pixels of the tile.
+//   sums[0][c] = sum dxn*x, sums[1][c] = sum dxn, sums[2][c] = sum dgam     (fp64, accumulated over the valid pixels)
+// Same mapping as the combine kernel: warp w owns channels w, w+8, ..., a lane owns 4 pixels of the tile.  The rows of
+// the last, partial tile past the image hold whatever their buffers hold (the producers of dpre and gam do not write
+// them): they are read as zero, so dxn and dgam are zero there and the sums see only the image.
 __global__ void __launch_bounds__(256) pixel_mod_bwd_kernel(const float* __restrict__ dpre, const float* __restrict__ x,
                                                             long x_bstride, const float* __restrict__ scsh,
                                                             float* __restrict__ gam_dgam, float* __restrict__ dxn,
-                                                            double* __restrict__ sums, int B, int T) {
+                                                            double* __restrict__ sums, int B, int T, int HW) {
   __shared__ float s_acc[3 * kWC];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int i = threadIdx.x; i < 3 * kWC; i += blockDim.x) s_acc[i] = 0.f;
@@ -486,12 +493,18 @@ __global__ void __launch_bounds__(256) pixel_mod_bwd_kernel(const float* __restr
     const int b = tile / T, ti = tile - b * T;
     const long off = static_cast<long>(tile) * kWC * 128 + lane * 4;
     const long xoff = static_cast<long>(b) * x_bstride + static_cast<long>(ti) * kWC * 128 + lane * 4;
+    const int nvalid = HW - ti * 128 - lane * 4;      // valid pixels among this lane's 4 (>= 4: all of them)
 #pragma unroll 4
     for (int c = warp; c < kWC; c += 8) {
       const float sc = scsh[c], sh = scsh[kWC + c];
-      const float4 d = __ldcs(reinterpret_cast<const float4*>(dpre + off + c * 128));
-      const float4 xv = __ldcs(reinterpret_cast<const float4*>(x + xoff + c * 128));
-      const float4 g = __ldcs(reinterpret_cast<const float4*>(gam_dgam + off + c * 128));
+      float4 d = __ldcs(reinterpret_cast<const float4*>(dpre + off + c * 128));
+      float4 xv = __ldcs(reinterpret_cast<const float4*>(x + xoff + c * 128));
+      float4 g = __ldcs(reinterpret_cast<const float4*>(gam_dgam + off + c * 128));
+      if (nvalid < 4) {
+        d = keep_first(d, nvalid);
+        xv = keep_first(xv, nvalid);
+        g = keep_first(g, nvalid);
+      }
       const float4 dx = make_float4(d.x * g.x, d.y * g.y, d.z * g.z, d.w * g.w);
       const float4 dg = make_float4(d.x * fmaf(xv.x, sc, sh), d.y * fmaf(xv.y, sc, sh), d.z * fmaf(xv.z, sc, sh),
                                     d.w * fmaf(xv.w, sc, sh));
@@ -710,7 +723,8 @@ int hg_spade_pixel_mod_bwd(const float* dpre, const float* x, long x_bstride, co
   const int T = (Hg * Wg + 127) / 128;
   int grid = hg::num_sms() * 4;
   if (grid > B * T) grid = B * T;
-  hg::pixel_mod_bwd_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(dpre, x, x_bstride, scsh, gam_dgam, dxn, sums, B, T);
+  hg::pixel_mod_bwd_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(dpre, x, x_bstride, scsh, gam_dgam, dxn, sums, B, T,
+                                                                                 Hg * Wg);
   return hg::check_launch("hg_spade_pixel_mod_bwd");
 }
 

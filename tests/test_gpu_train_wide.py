@@ -33,38 +33,79 @@ def _rel(a, b):
 # ----------------------------------------------------------------------------------------------------------------------
 # 1. kernel: operand scale over K = 512
 # ----------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("act,K", [(0, 512), (1, 512), (1, 256)])
-def test_conv_bwd_operand_scale(act, K):
+def _multi_tile_shape():
+    """(B, Hg, Wg) with T < SMs tiles per sample and B*T >= 2 SMs tiles: every persistent CTA walks tiles of several
+    samples, so the per-sample [B,2,C] sums are flushed mid-CTA."""
+    n = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+    Wg = 100
+    Hg = (n // 3 + 1) * 128 // Wg
+    T = (Hg * Wg + 127) // 128
+    return -(-2 * n // T) + 1, Hg, Wg
+
+
+# the pixel-major Cout = 128 epilogue as synthesis_train.synthesis_backward calls it for the gamma/beta MLP: no table, no
+# operand scale, the ReLU mask (slope 0) of A1
+_PM = dict(cout=128, pm=True, slope=0.0, ascale=False, mod=False)
+
+
+@pytest.mark.parametrize("act,K,case", [
+    pytest.param(0, 512, {}, id="0-512"),
+    pytest.param(1, 512, {}, id="1-512"),
+    pytest.param(1, 256, {}, id="1-256"),
+    pytest.param(0, 512, _PM, id="pixel-major-cout128-relu"),
+    pytest.param(0, 512, dict(_PM, shape="multi"), id="pixel-major-cout128-relu-multi"),
+    pytest.param(0, 256, dict(slope=0.0), id="relu-K256"),
+    pytest.param(0, 512, dict(ascale=False), id="lrelu-K512-noascale"),
+    pytest.param(1, 512, dict(rk_n=1), id="sine-K512-rk1"),
+    pytest.param(1, 256, dict(rk_n=2, ascale=False), id="sine-K256-rk2-noascale"),
+    pytest.param(0, 512, dict(shape="multi"), id="lrelu-K512-multi"),
+    pytest.param(1, 256, dict(shape="multi", rk_n=1), id="sine-K256-rk1-multi"),
+    pytest.param(0, 512, dict(shape=(2, 12, 26)), id="lrelu-K512-last56"),
+])
+def test_conv_bwd_operand_scale(act, K, case):
     abi = importlib.import_module("3dhumangan_b200.abi")
-    B, Hg, Wg = 2, 16, 20
+    shape = case.get("shape", (2, 16, 20))
+    B, Hg, Wg = _multi_tile_shape() if shape == "multi" else shape
+    cout, slope = case.get("cout", 256), case.get("slope", 0.2)
+    rk_n = case.get("rk_n", 3) if act == 1 else 0
     HW = Hg * Wg
     g = torch.Generator().manual_seed(31 + act + K)
     go = torch.randn(B, K, HW, generator=g)
-    aux = torch.randn(B, 256, HW, generator=g)
+    aux = torch.randn(B, cout, HW, generator=g)
+    if not case.get("mod", True):
+        aux = torch.relu(aux)                                   # A1 = relu(...): exact zeros where the mask is 0
     W = torch.randn(K, 256, generator=g) / 16                   # forward weight [K outputs, 256 inputs]
-    ascale = 1.0 + 0.5 * torch.randn(B, K, generator=g)
-    mod = torch.stack([1.0 + 0.5 * torch.randn(B, 256, generator=g), 0.5 * torch.randn(B, 256, generator=g)], dim=1)
-    dy = torch.einsum("oc,bop->bcp", W.double(), go.double() * ascale.double()[:, :, None])
+    W[:, cout:] = 0                                             # the MMA runs N = 256; rows past Cout of W^T are zero
+    ascale = 1.0 + 0.5 * torch.randn(B, K, generator=g) if case.get("ascale", True) else None
+    mod = None
+    if case.get("mod", True):
+        mod = torch.stack([1.0 + 0.5 * torch.randn(B, cout, generator=g), 0.5 * torch.randn(B, cout, generator=g)], dim=1)
+    gs = go.double() if ascale is None else go.double() * ascale.double()[:, :, None]
+    dy = torch.einsum("oc,bop->bcp", W[:, :cout].double(), gs)
     rk_w = rk_v = None
-    if act == 1:                # rank-3 head term
-        rk_w = torch.randn(3, 256, generator=g)
-        rk_v = torch.randn(B, 3, HW, generator=g)
-        dy = dy + torch.einsum("jc,bjp->bcp", rk_w.double(), rk_v.double())
-    pre = aux.double() * mod[:, 0, :, None].double() + mod[:, 1, :, None].double()
-    ref = dy * (torch.cos(pre) if act == 1 else torch.where(pre > 0, 1.0, 0.2))
+    if rk_n:                    # rank-k head term; rows of the [3,C] weight past rk_n are zero
+        rk_w = torch.zeros(3, 256)
+        rk_w[:rk_n] = torch.randn(rk_n, 256, generator=g)
+        rk_v = torch.randn(B, rk_n, HW, generator=g)
+        dy = dy + torch.einsum("jc,bjp->bcp", rk_w.double(), torch.cat([rk_v.double(), torch.zeros(B, 3 - rk_n, HW).double()], 1))
+    pre = aux.double() if mod is None else aux.double() * mod[:, 0, :, None].double() + mod[:, 1, :, None].double()
+    ref = dy * (torch.cos(pre) if act == 1 else torch.where(pre > 0, 1.0, slope))
     s1, s2 = ref.sum(2), (ref * aux.double()).sum(2)
 
     wimg_t, _ = abi.pack_weight(W.t().contiguous().cuda(), Nb=256)
     gb = _blocked(go).cuda()
-    out = torch.full((B, gb.shape[1], 256, 128), float("nan"), device="cuda")
-    sums = torch.zeros(B, 2, 256, dtype=torch.float64, device="cuda")
+    T = gb.shape[1]
+    out = torch.full((B, HW, cout) if case.get("pm") else (B, T, cout, 128), float("nan"), device="cuda")
+    sums = torch.zeros(B, 2, cout, dtype=torch.float64, device="cuda")
     abi.conv1x1_blocked_bwd(gb[:, :, :256].contiguous(), _blocked(aux).cuda(), wimg_t, out, sums,
-                            g2=gb[:, :, 256:].contiguous() if K == 512 else None, mod=mod.cuda(), act=act,
-                            ascale=ascale.cuda().contiguous(), rk_w=None if rk_w is None else rk_w.cuda(),
-                            rk_v=None if rk_v is None else rk_v.cuda(), B=B, Hg=Hg, Wg=Wg)
+                            g2=gb[:, :, 256:].contiguous() if K == 512 else None, mod=None if mod is None else mod.cuda(), act=act,
+                            ascale=None if ascale is None else ascale.cuda().contiguous(), rk_w=None if rk_w is None else rk_w.cuda(),
+                            rk_v=None if rk_v is None else rk_v.cuda(), Cout=cout, slope=slope, pixel_major=case.get("pm", False),
+                            B=B, Hg=Hg, Wg=Wg)
     torch.cuda.synchronize()
-    got = _planar(out, HW).cpu().double()
-    safe = pre.abs() > 1e-5 if act == 0 else torch.ones_like(pre, dtype=torch.bool)
+    got = (out.permute(0, 2, 1) if case.get("pm") else _planar(out, HW)).cpu().double()
+    # pre-activations within rounding distance of zero may pick the other side of the mask (without a table pre is exact)
+    safe = pre.abs() > 1e-5 if act == 0 and mod is not None else torch.ones_like(pre, dtype=torch.bool)
     assert ((got - ref) * safe).abs().max() / ref.abs().max() < 5e-5
     assert (sums[:, 0].cpu() - s1).abs().max() / s1.abs().max() < 5e-4
     assert (sums[:, 1].cpu() - s2).abs().max() / s2.abs().max() < 5e-4
