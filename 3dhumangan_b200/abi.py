@@ -79,6 +79,9 @@ SIGNATURES = {
     "hg_seg_ce_coef": (c_int, [c_void_p, c_void_p, c_int, c_double, c_void_p, c_void_p]),
     "hg_seg_ce": (c_int, [c_void_p] * 6 + [c_int, c_int, c_long, c_void_p]),
     "hg_image_loss": (c_int, [c_void_p] * 6 + [c_int, c_long, c_int, c_float, c_void_p]),
+    "hg_latent_pool_gather": (c_int, [c_void_p, c_long, c_int, c_void_p, c_int, c_void_p, c_void_p]),
+    "hg_latent_pool_grad": (c_int, [c_void_p, c_void_p, c_int, c_int, c_long, c_void_p, c_void_p]),
+    "hg_latent_loss": (c_int, [c_void_p, c_void_p, c_int, c_int, c_float, c_void_p, c_void_p, c_void_p, c_void_p]),
     "hg_vgg_input": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p]),
     "hg_vgg_input_adjoint": (c_int, [c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p]),
     "hg_maxpool2x2": (c_int, [c_void_p, c_void_p, c_long, c_int, c_int, c_void_p]),

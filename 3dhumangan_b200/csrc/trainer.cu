@@ -116,8 +116,9 @@ __global__ void sum_partials_kernel(const double* __restrict__ partials, int n, 
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// image reconstruction loss: mean over the B*3*HW elements of m[b,p] * rho(pred - target), rho(d) = d^2 (mode 0) or the
-// Charbonnier sqrt(d^2 + eps^2) (mode 1; eps -> 0 is L1), and its gradient, in one pass.  fp64 partial per block.
+// image reconstruction loss: mean over the B*3*HW elements of m[b,p] * rho(pred - target), rho(d) = d^2 (mode 0), the
+// Charbonnier sqrt(d^2 + eps^2) (mode 1; eps -> 0 is L1) or smooth L1 with beta = eps (mode 2: the photometric loss of
+// phase_trainer.py:525-527), and its gradient, in one pass.  fp64 partial per block.
 // ------------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) image_loss_kernel(const float* __restrict__ pred, const float* __restrict__ target,
                                                          const float* __restrict__ mask, int mode, float eps, float scale,
@@ -132,9 +133,18 @@ __global__ void __launch_bounds__(256) image_loss_kernel(const float* __restrict
     if (mode == 0) {
       rho = d * d;
       drho = 2.f * d;
-    } else {
+    } else if (mode == 1) {
       rho = sqrtf(fmaf(d, d, eps * eps));
       drho = d / rho;
+    } else {                                        // F.smooth_l1_loss(beta = eps)
+      const float z = fabsf(d);
+      if (z < eps) {
+        rho = 0.5f * z * z / eps;
+        drho = d / eps;
+      } else {
+        rho = z - 0.5f * eps;
+        drho = d > 0.f ? 1.f : -1.f;
+      }
     }
     acc += static_cast<double>(m * rho);
     if (dpred) __stcs(dpred + e, m * drho * scale);
@@ -285,7 +295,8 @@ int hg_image_loss(const float* pred, const float* target, const float* mask, flo
                   int B, long HW, int mode, float eps, void* stream) {
   HG_REQUIRE(pred && target && loss && workspace, "hg_image_loss: null pointer");
   HG_REQUIRE(B > 0 && HW > 0, "hg_image_loss: bad shape");
-  HG_REQUIRE(mode == 0 || (mode == 1 && eps > 0.f), "hg_image_loss: mode 0 (L2) or 1 (Charbonnier, eps > 0)");
+  HG_REQUIRE(mode == 0 || ((mode == 1 || mode == 2) && eps > 0.f),
+             "hg_image_loss: mode 0 (L2), 1 (Charbonnier, eps > 0) or 2 (smooth L1, beta = eps > 0)");
   auto st = static_cast<cudaStream_t>(stream);
   const long total = static_cast<long>(B) * 3 * HW;
   long blocks = (total + 255) / 256;

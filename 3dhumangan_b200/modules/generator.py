@@ -44,7 +44,8 @@ def _precision_passes(kwargs=None):
 # parameter holders with the reference's names
 # ------------------------------------------------------------------------------------------------
 class LatentPool(nn.Module):
-    """lib/components/util.py:18-29."""
+    """lib/components/util.py:18-29.  On CUDA the lookup and its dense gradient run on hg_latent_pool_gather /
+    hg_latent_pool_grad (`ops.trainer_ops.latent_pool_gather`); a CPU pool is indexed by torch."""
 
     def __init__(self, pool_size, latent_dim):
         super().__init__()
@@ -55,6 +56,9 @@ class LatentPool(nn.Module):
             self.latents.copy_(latents)
 
     def forward(self, indices):
+        if self.latents.is_cuda:
+            from ..ops.trainer_ops import latent_pool_gather
+            return latent_pool_gather(self.latents, torch.as_tensor(indices))
         return self.latents[indices]
 
 

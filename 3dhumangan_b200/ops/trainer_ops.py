@@ -2,8 +2,11 @@
 
   seg_ce_balanced   PhaseTrainer._calculate_segmentation_loss, mode 'cross_entropy_balanced' (phase_trainer.py:203-256):
                     label histogram -> per-class coefficients -> ONE pass over the logits that yields the loss and its gradient.
-  image_loss        reconstruction loss of latent inversion (inversion.py): weighted L2 or Charbonnier over an image, value
-                    and gradient in one pass.
+  image_loss        reconstruction loss of latent inversion (inversion.py) and the photometric loss of conditional phases
+                    (phase_trainer.py:525-527): weighted L2, Charbonnier or smooth L1 over an image, value and gradient in one pass.
+  latent_pool_gather  `LatentPool.forward` (lib/components/util.py:18-29) with the dense [P,L] gradient of `latents[indices]`.
+  latent_loss       the latent regression of phase_trainer.py:425-437, :493-506: mean SL1_beta(n(pred) - n(target)),
+                    n = normalize_2nd_moment.
   FusedAdam         torch.optim.Adam (same state_dict: step / exp_avg / exp_avg_sq, same arithmetic) for the reference's
                     parameter groups (phase_trainer.py:57-76) with global-norm clipping (clip_grad_norm_, :314,336) and the
                     generator's EMA (lib/components/ema.py:29-48) folded into the same multi-tensor launch.
@@ -101,16 +104,104 @@ class _ImageLoss(torch.autograd.Function):
         return (dpred * g if dpred is not None else None), None, None, None, None
 
 
-def image_loss(pred, target, mask=None, kind="l2", eps=1e-3):
-    """mean over the B*3*H*W elements of mask * rho(pred - target): rho(d) = d^2 (`kind="l2"`) or the Charbonnier
-    sqrt(d^2 + eps^2) (`kind="charbonnier"`, a smooth L1).  `mask` [B,1,H,W] fp32 weights each pixel (the person's
+def image_loss(pred, target, mask=None, kind="l2", eps=1e-3, beta=1.0):
+    """mean over the B*3*H*W elements of mask * rho(pred - target): rho(d) = d^2 (`kind="l2"`), the Charbonnier
+    sqrt(d^2 + eps^2) (`kind="charbonnier"`) or `F.smooth_l1_loss`'s rho with `beta` (`kind="smooth_l1"`, the photometric
+    loss of phase_trainer.py:525-527 with beta = 0.1).  `mask` [B,1,H,W] fp32 weights each pixel (the person's
     silhouette: `preprocess.Preprocessor` labels != background) or None.  Differentiable w.r.t. `pred` (first order); the
     value repeats bit for bit (fp64 partial sums in a fixed order)."""
-    if kind not in ("l2", "charbonnier"):
-        raise RuntimeError(f"hg3d: image_loss kind {kind!r} is not built ('l2' or 'charbonnier')")
+    modes = {"l2": (0, eps), "charbonnier": (1, eps), "smooth_l1": (2, beta)}
+    if kind not in modes:
+        raise RuntimeError(f"hg3d: image_loss kind {kind!r} is not built ('l2', 'charbonnier' or 'smooth_l1')")
     if mask is not None:
         mask = mask.to(torch.float32)
-    return _ImageLoss.apply(pred, target, mask, 0 if kind == "l2" else 1, eps)
+    mode, e = modes[kind]
+    return _ImageLoss.apply(pred, target, mask, mode, e)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# latent pool lookup and latent regression
+# ----------------------------------------------------------------------------------------------------------------------
+class _LatentPoolGather(torch.autograd.Function):
+    @staticmethod
+    @torch.amp.custom_fwd(device_type="cuda", cast_inputs=torch.float32)
+    def forward(ctx, pool, indices):
+        abi.require_device()
+        if pool.dim() != 2 or indices.dim() != 1 or indices.dtype != torch.int64:
+            raise RuntimeError("hg3d: latent_pool_gather expects a pool [P,L] and int64 indices [B]")
+        pool = pool.contiguous()
+        indices = indices.to(pool.device).contiguous()
+        P, L = pool.shape
+        B = indices.shape[0]
+        out = torch.empty(B, L, dtype=torch.float32, device=pool.device)
+        if B > 0:
+            with torch.cuda.device_of(pool):
+                abi.call("hg_latent_pool_gather", abi.ptr(pool), P, L, abi.ptr(indices), B, abi.ptr(out), abi.stream())
+        ctx.save_for_backward(indices)
+        ctx.pool_shape = (P, L)
+        return out
+
+    @staticmethod
+    @torch.amp.custom_bwd(device_type="cuda")
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, dz):
+        (indices,) = ctx.saved_tensors
+        P, L = ctx.pool_shape
+        dz = dz.float().contiguous()
+        dpool = torch.empty(P, L, dtype=torch.float32, device=dz.device)
+        with torch.cuda.device_of(dz):
+            if indices.shape[0] > 0:
+                abi.call("hg_latent_pool_grad", abi.ptr(dz), abi.ptr(indices), indices.shape[0], L, P, abi.ptr(dpool), abi.stream())
+            else:
+                dpool.zero_()
+        return dpool, None
+
+
+def latent_pool_gather(pool, indices):
+    """`pool[indices]` for a pool [P,L] (the `latent_pool.latents` parameter) and integer indices [B] -> [B,L].  The backward
+    returns the dense [P,L] gradient that the reference's `self.latents[indices]` produces -- zero rows except the indexed
+    ones, each the sum of its rows of the incoming gradient in batch order -- to autograd, so accumulation over micro-batches
+    and DDP's reducer hooks treat it as any other parameter's gradient.  An index outside [0, P) gives a NaN row."""
+    idx = indices.long()
+    return _LatentPoolGather.apply(pool, idx.reshape(-1)).reshape(*idx.shape, pool.shape[-1])
+
+
+class _LatentLoss(torch.autograd.Function):
+    @staticmethod
+    @torch.amp.custom_fwd(device_type="cuda", cast_inputs=torch.float32)
+    def forward(ctx, pred, target, beta):
+        abi.require_device()
+        if pred.dim() != 2 or target.shape != pred.shape:
+            raise RuntimeError("hg3d: latent_loss expects prediction and target [B,L] of one shape")
+        pred, target = pred.contiguous(), target.contiguous()
+        loss = torch.empty(1, dtype=torch.float32, device=pred.device)
+        with torch.cuda.device_of(pred):
+            abi.call("hg_latent_loss", abi.ptr(pred), abi.ptr(target), pred.shape[0], pred.shape[1], float(beta), None, None, abi.ptr(loss),
+                     abi.stream())
+        ctx.save_for_backward(pred, target)
+        ctx.beta = beta
+        return loss.reshape(())
+
+    @staticmethod
+    @torch.amp.custom_bwd(device_type="cuda")
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g):
+        pred, target = ctx.saved_tensors
+        if not ctx.needs_input_grad[0]:
+            return None, None, None
+        dpred = torch.empty_like(pred)
+        g = g.float().reshape(1).contiguous()
+        with torch.cuda.device_of(pred):
+            abi.call("hg_latent_loss", abi.ptr(pred), abi.ptr(target), pred.shape[0], pred.shape[1], float(ctx.beta), abi.ptr(g),
+                     abi.ptr(dpred), None, abi.stream())
+        return dpred, None, None
+
+
+def latent_loss(pred, target, beta=0.1):
+    """`F.smooth_l1_loss(normalize_2nd_moment(pred), normalize_2nd_moment(target), beta=beta)` for [B,L] latents
+    (phase_trainer.py:425-437, :493-506) -> scalar; differentiable w.r.t. `pred` (first order), `target` is a constant.
+    The value repeats bit for bit (fp64 row sums in a fixed order)."""
+    return _LatentLoss.apply(pred, target.detach(), beta)
 
 
 # ----------------------------------------------------------------------------------------------------------------------

@@ -136,3 +136,23 @@ def make_conditions(batch_size: int, seed: int = 1, pose_std: float = 0.3, view_
         "intrinsics": f32(K),
         "scales": f32(torch.full((B,), scale, dtype=torch.float64)),
     }
+
+
+def make_appearance(batch_size: int, dataset_length: int, latent_dim: int, seed: int = 1, repeats: bool = False, device="cpu"):
+    """-> (codes [dataset_length, latent_dim], {"indices": int64 [B], "latents": [B, latent_dim]}): stand-ins for the per-image
+    inversion codes that seed `latent_pool` (`get_all_latents`, phase_trainer.py:29-32) and for the `indices` / `latents` items
+    of a batch (lib/data/datasets.py:291), to be merged into the `conditions` dict of a conditional phase.  `latents` are the
+    batch's rows of `codes`.  repeats=True draws about half as many distinct images as the batch holds, so that indices repeat
+    (in shuffled order); otherwise the indices are distinct (batch_size <= dataset_length)."""
+    gen = torch.Generator().manual_seed(seed)
+    codes = torch.randn(dataset_length, latent_dim, generator=gen)
+    if repeats:
+        distinct = torch.randperm(dataset_length, generator=gen)[:max(1, (batch_size + 1) // 2)]
+        idx = distinct[torch.randint(0, distinct.numel(), (batch_size,), generator=gen)]
+        idx[:distinct.numel()] = distinct[:batch_size]
+        idx = idx[torch.randperm(batch_size, generator=gen)]
+    else:
+        if batch_size > dataset_length:
+            raise ValueError("hg3d: distinct indices need batch_size <= dataset_length")
+        idx = torch.randperm(dataset_length, generator=gen)[:batch_size]
+    return codes.to(device), {"indices": idx.to(device), "latents": codes[idx].contiguous().to(device)}

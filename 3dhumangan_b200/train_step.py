@@ -55,6 +55,19 @@ def segmentation_loss(segments, gt, label_dim, prior_weights=None, with_stats=Fa
     return loss, acc, real_prob
 
 
+def normalize_2nd_moment(x, dim=1, eps=1e-8):
+    """lib/components/util.py:58."""
+    return x * (x.square().mean(dim=dim, keepdim=True) + eps).rsqrt()
+
+
+def latent_regression_loss(pred, target):
+    """The latent term of phase_trainer.py:425-437 and :493-506 for one side: SL1_0.1(n(pred), n(target)), the target under
+    no_grad."""
+    with torch.no_grad():
+        target = normalize_2nd_moment(target)
+    return F.smooth_l1_loss(normalize_2nd_moment(pred), target, beta=0.1)
+
+
 def r1_penalty(disc_input_real, out_real, scaler, meta):
     """phase_trainer.py:259-294, arithmetic as the reference EXECUTES it: the gradient of f = sum(prediction) (gan_lambda > 0) or
     sum(softmax(segments)) (segmentation only) w.r.t. the real images is taken for the whole batch, but
@@ -186,16 +199,30 @@ class Trainer:
 
     `batch`: dict(images [B,3,H,W], labels [B,H,W] int64 (the real segmentation map), cond = the pose conditions,
     optional z_d / z_g latents (drawn like `z_sampler` otherwise)).  `meta` is the merged curriculum dict that the
-    reference splats into every call."""
+    reference splats into every call.  Conditional phases (`uncond: False`) and `latent_lambda > 0` also read
+    `cond["indices"]` (int64 [B], the images' rows of `generator.latent_pool`) and `cond["latents"]` ([B, latent_dim], their
+    inversion codes), the `indices` / `latents` of the reference's dataset (lib/data/datasets.py:291)."""
 
-    def __init__(self, G, D, meta, *, amp=None, ddp=None, amp_dtype=torch.float16, ema_decay=0.999, fused=True, preprocessor=None):
+    def __init__(self, G, D, meta, *, amp=None, ddp=None, amp_dtype=torch.float16, ema_decay=0.999, fused=True, preprocessor=None,
+                 perceptual=None, appearance_codes=None):
         """fused=True: the loss / clipping / Adam / EMA tail on the sm_90a kernels of csrc/trainer.cu (ops.trainer_ops);
         fused=False: the same steps as torch calls (F.cross_entropy, clip_grad_norm_, torch.optim.Adam, foreach lerp).
         preprocessor: a `preprocess.Preprocessor`.  With one, each step draws a view for `batch["cond"]` as
         phase_trainer.py:305,329 do, and the segmentation targets follow :350-353 and :533 -- the rasterised map on rotate phases,
         otherwise the rasterised map or `batch["labels"]` (the dataset's body_segments) with probability 1/2 each, drawn with
-        `random.random()`.  Without one, `batch["cond"]` is used as given and `batch["labels"]` is the target in every phase."""
+        `random.random()`.  Without one, `batch["cond"]` is used as given and `batch["labels"]` is the target in every phase.
+        perceptual: the module of the perceptual term of conditional phases (`perceptual.VGGPerceptualLoss` or any module with
+        its `forward(input, target)` -> 4 losses); built from torchvision's cached VGG16 weights when `sum(perceptual_lambda) > 0`
+        and none is given (phase_trainer.py:51-54; raises when the weights are missing, nothing is downloaded).
+        appearance_codes: [P, latent_dim] initial `generator.latent_pool` rows, the dataset's inversion codes
+        (phase_trainer.py:29-32)."""
         self.preprocessor = preprocessor
+        if appearance_codes is not None:
+            G.latent_pool.init(torch.as_tensor(appearance_codes))
+        if perceptual is None and sum(meta.get("perceptual_lambda", [0])) > 0:
+            from .perceptual import VGGPerceptualLoss
+            perceptual = VGGPerceptualLoss().to(next(G.parameters()).device)
+        self.perceptual = perceptual
         import torch.distributed as dist
         self.meta = dict(meta)
         self.fused = bool(fused)
@@ -225,6 +252,18 @@ class Trainer:
             from .ops.trainer_ops import seg_ce_balanced
             return seg_ce_balanced(segments, gt, self.meta["label_dim"], self.meta.get("segmentation_weights"))
         return segmentation_loss(segments, gt, self.meta["label_dim"], self.meta.get("segmentation_weights"))
+
+    def _latent_loss(self, pred, target):
+        if self.fused:
+            from .ops.trainer_ops import latent_loss
+            return latent_loss(pred, target, beta=0.1)
+        return latent_regression_loss(pred, target)
+
+    def _photometric_loss(self, rgbs, images):
+        if self.fused:
+            from .ops.trainer_ops import image_loss
+            return image_loss(rgbs, images.detach(), kind="smooth_l1", beta=0.1)
+        return F.smooth_l1_loss(rgbs, images.detach(), beta=0.1)
 
     def _optimizer_step(self, opt, params, ema=None):
         """unscale_ -> clip_grad_norm_ -> scaler.step (-> EMA): phase_trainer.py:313-316, 335-339."""
@@ -258,9 +297,9 @@ class Trainer:
     def _check_phase(self, phase):
         """The input selection of `_get_disc_input_real / _gen` (phase_trainer.py:162-200) has two more branches (dual discrimination,
         render-resolution modalities) that no shipped curriculum reaches: refuse them instead of training on the wrong tensors."""
-        if self.meta.get("dual_discrimination", False) or "render" in phase["gen_modal"] or not phase.get("uncond", True):
-            raise RuntimeError("hg3d: dual_discrimination / gen_modal '%s' / conditional phases are not used by any shipped "
-                               "curriculum and are not built" % phase["gen_modal"])
+        if self.meta.get("dual_discrimination", False) or "render" in phase["gen_modal"]:
+            raise RuntimeError("hg3d: dual_discrimination / gen_modal '%s' are not used by any shipped curriculum and are not "
+                               "built" % phase["gen_modal"])
 
     def train_discriminator(self, batch, alpha=1.0):
         meta, phase = self.meta, self._phase()
@@ -272,6 +311,7 @@ class Trainer:
             if phase["rotate"] or random.random() < 0.5:
                 labels = cond["rasterized_segments"]
         B = real_images.shape[0]
+        uncond = phase.get("uncond", True)
         with self._autocast():
             with torch.no_grad():
                 z = self._z(batch, "z_d", B, real_images.device)
@@ -279,7 +319,8 @@ class Trainer:
                 outs = []
                 for s in range(self.batch_split):
                     sl = slice(s * split, (s + 1) * split)
-                    outs.append(self.generator_ddp(z[sl], {k: v[sl] for k, v in cond.items()}, latent_indices=None, **meta))
+                    sub = {k: v[sl] for k, v in cond.items()}
+                    outs.append(self.generator_ddp(z[sl], sub, latent_indices=None if uncond else sub["indices"], **meta))
                 gen_outputs = {k: torch.cat([o[k] for o in outs], 0) for k in outs[0]}
             disc_input_real = real_images.detach().clone() if real_images.requires_grad else real_images
             disc_input_real.requires_grad = True
@@ -299,9 +340,13 @@ class Trainer:
                        + self._seg_loss(out_gen["segments"], torch.zeros_like(labels))) * meta["segmentation_lambda"]
             else:
                 seg = (out_real["segments"].sum() + out_gen["segments"].sum()) * 0
-            latent_loss = (out_real["latents"].sum() + out_gen["latents"].sum()) * 0      # latent_lambda = 0 in every shipped curriculum
-            if meta.get("latent_lambda", 0) > 0:
-                raise RuntimeError("hg3d: latent_lambda > 0 is not used by any shipped curriculum and is not built")
+            if meta.get("latent_lambda", 0) > 0:          # phase_trainer.py:425-437
+                with torch.no_grad():
+                    gt_gen = z if uncond else self.generator.latent_pool(cond["indices"])
+                latent_loss = (self._latent_loss(out_gen["latents"], gt_gen)
+                               + self._latent_loss(out_real["latents"], cond["latents"])) * meta["latent_lambda"]
+            else:
+                latent_loss = (out_real["latents"].sum() + out_gen["latents"].sum()) * 0
             d_loss = gan_loss + grad_penalty + seg + latent_loss
         self.scaler.scale(d_loss).backward()
         self._optimizer_step(self.optimizer_D, list(self.discriminator_ddp.parameters()))
@@ -316,6 +361,7 @@ class Trainer:
         if self.preprocessor is not None:
             cond = self.preprocessor(dict(cond), phase["rotate"], **meta)
         B = real_images.shape[0]
+        uncond = phase.get("uncond", True)
         z = self._z(batch, "z_g", B, real_images.device)
         split = B // self.batch_split
         total = 0.0
@@ -332,12 +378,27 @@ class Trainer:
                 sl = slice(s * split, (s + 1) * split)
                 with self._autocast():
                     sub = {k: v[sl] for k, v in cond.items()}
-                    gen_outputs = self.generator_ddp(z[sl], sub, latent_indices=None, **meta)
-                    out = self.discriminator(gen_outputs[phase["gen_modal"]], sub, alpha=alpha, mode="gen", **meta)
+                    gen_outputs = self.generator_ddp(z[sl], sub, latent_indices=None if uncond else sub["indices"], **meta)
+                    rgbs = gen_outputs[phase["gen_modal"]]
+                    out = self.discriminator(rgbs, sub, alpha=alpha, mode="gen", **meta)
                     pred_gen = out["prediction"]
-                    gan_lambda = meta["gan_lambda"] if phase["uncond"] else 0
+                    gan_lambda = meta["gan_lambda"] if uncond else 0
                     gan_loss = gan_lambda * F.softplus(-pred_gen).mean() if gan_lambda > 0 else 0 * pred_gen.sum()
-                    latent_loss = out["latents"].sum() * 0
+                    if meta.get("latent_lambda", 0) > 0:          # phase_trainer.py:493-506
+                        with torch.no_grad():
+                            gt = z[sl] if uncond else self.generator.latent_pool(sub["indices"])
+                        latent_loss = self._latent_loss(out["latents"], gt)
+                        if not uncond:        # depends on no parameter; part of the reported loss as in the reference
+                            latent_loss = latent_loss + F.smooth_l1_loss(z[sl], sub["latents"].detach(), beta=0.1)
+                        latent_loss = latent_loss * meta["latent_lambda"]
+                    else:
+                        latent_loss = out["latents"].sum() * 0
+                    g_loss = gan_loss          # + the perceptual and photometric terms of conditional phases (:509-527)
+                    if not uncond and sum(meta.get("perceptual_lambda", [0])) > 0:
+                        losses = self.perceptual(0.5 * rgbs + 0.5, (0.5 * real_images[sl] + 0.5).detach())
+                        g_loss = g_loss + sum(meta["perceptual_lambda"][i] * losses[i] for i in range(4))
+                    if not uncond and meta.get("photometric_lambda", 0) > 0:
+                        g_loss = g_loss + self._photometric_loss(rgbs, real_images[sl]) * meta["photometric_lambda"]
                     if meta["segmentation_lambda"] > 0:
                         gt = labels[sl]
                         if self.preprocessor is not None and (phase["rotate"] or random.random() < 0.5):
@@ -345,7 +406,7 @@ class Trainer:
                         seg = self._seg_loss(out["segments"], gt) * meta["segmentation_lambda"]
                     else:
                         seg = out["segments"].sum() * 0
-                    g_loss = (gan_loss + latent_loss + seg) / self.batch_split
+                    g_loss = (g_loss + latent_loss + seg) / self.batch_split
                     self.scaler.scale(g_loss).backward()
                 total = total + g_loss.detach()
         finally:

@@ -322,11 +322,28 @@ int hg_label_histogram(const long* labels, long n, int L, int* hist, void* strea
 int hg_seg_ce_coef(const int* hist, const float* prior /* [L] or NULL */, int L, double numel, float* coef, void* stream);
 int hg_seg_ce(const float* logits, const long* labels, const float* coef, float* dlogits /* or NULL */, float* loss,
               double* workspace /* >= 2 * #SMs doubles */, int B, int L, long HW, void* stream);
-/* Image reconstruction loss of latent inversion: loss[0] = mean over the B*3*HW elements of mask[b,p] * rho(pred - target),
- * rho(d) = d^2 (mode 0) or the Charbonnier sqrt(d^2 + eps^2) (mode 1), and optionally d loss / d pred, in one pass; fp64
- * block partials summed in a fixed order.  pred / target [B,3,HW], mask [B,HW] or NULL (all ones). */
+/* Image reconstruction loss: loss[0] = mean over the B*3*HW elements of mask[b,p] * rho(pred - target), rho(d) = d^2
+ * (mode 0), the Charbonnier sqrt(d^2 + eps^2) (mode 1, latent inversion) or F.smooth_l1_loss with beta = eps (mode 2, the
+ * photometric loss of a conditional generator step, phase_trainer.py:525-527), and optionally d loss / d pred, in one pass;
+ * fp64 block partials summed in a fixed order.  pred / target [B,3,HW], mask [B,HW] or NULL (all ones). */
 int hg_image_loss(const float* pred, const float* target, const float* mask, float* dpred /* or NULL */, float* loss,
                   double* workspace /* >= 2 * #SMs doubles */, int B, long HW, int mode, float eps, void* stream);
+/* Conditional (reconstruction) phases of PhaseTrainer (lib/trainers/phase_trainer.py:344-553).
+ * hg_latent_pool_gather: out [B,L] = pool [P,L] rows idx[b] (int64 [B]): `LatentPool.forward` = `latents[indices]`
+ *                        (lib/components/util.py:18-29, looked up at phase_trainer.py:370-373, :466-468); a row whose index is
+ *                        outside [0, P) is written as NaN.
+ * hg_latent_pool_grad  : dpool [P,L] = the dense gradient of that lookup: zero except rows idx[b], each the fp64 sum of its dz
+ *                        [B,L] rows in batch order, rounded once, written by the block of the row's first occurrence (no atomics:
+ *                        repeats bit for bit).  Indices outside [0, P) contribute nothing.
+ * hg_latent_loss       : loss[0] = mean over B*L of smooth_l1_beta(n(pred) - n(target)), n = normalize_2nd_moment
+ *                        (lib/components/util.py:58: x * rsqrt(mean(x^2, dim=1) + 1e-8)) -- the latent regression of
+ *                        phase_trainer.py:425-437 (discriminator) and :493-506 (generator); dpred (optional) = gscale[0] (a
+ *                        device scalar, NULL: 1) * d loss / d pred through the normalisation's Jacobian.  loss may be NULL when
+ *                        dpred is not.  One block; fp64 row sums added in a fixed order. */
+int hg_latent_pool_gather(const float* pool, long P, int L, const long* idx, int B, float* out, void* stream);
+int hg_latent_pool_grad(const float* dz, const long* idx, int B, int L, long P, float* dpool, void* stream);
+int hg_latent_loss(const float* pred, const float* target, int B, int L, float beta, const float* gscale /* or NULL */,
+                   float* dpred /* or NULL */, float* loss /* or NULL */, void* stream);
 /* Multi-tensor global-norm clipping (torch.nn.utils.clip_grad_norm_, phase_trainer.py:314,336), torch.optim.Adam's update
  * with per-group scalars (phase_trainer.py:57-76) and the generator's EMA (lib/components/ema.py:29-48) over a device table
  * of tensors: entries { float* p, g, exp_avg, exp_avg_sq, ema; long n } (hg_mt_entry_bytes() = 48; g NULL = no gradient this
