@@ -32,6 +32,10 @@ SIGNATURES = {
     "hg_sample_fine": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_float, c_int] + [c_void_p] * 4 + [c_int] * 4
                        + [c_void_p] * 3),
     "hg_merge_samples": (c_int, [c_void_p] * 4 + [c_int] * 3 + [c_void_p] * 4),
+    "hg_iso_workspace_bytes": (c_size_t, [c_int, c_int, c_int]),
+    "hg_iso_count": (c_int, [c_void_p, c_int, c_int, c_int, c_float, c_void_p, c_size_t, c_void_p, c_void_p]),
+    "hg_iso_emit": (c_int, [c_void_p, c_int, c_int, c_int] + [c_float] * 5 + [c_void_p, c_size_t, ctypes.c_longlong]
+                    + [c_void_p] * 4),
     "hg_spade_conv": (c_int, [c_void_p, c_long, c_void_p, c_void_p, c_void_p, c_long] + [c_void_p] * 12 + [c_int] * 7 + [c_void_p]),
     "hg_bn_finalize": (c_int, [c_void_p, c_double, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_float, c_float,
                                c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
@@ -608,3 +612,36 @@ def dense(x, w, bias):
     with torch.cuda.device_of(x):
         call("hg_dense", ptr(x), ptr(w), ptr(bias), ptr(out), B, K, O, stream())
     return out
+
+
+def iso_surface(lattice, level, origin=(0.0, 0.0, 0.0), spacing=1.0):
+    """Marching-tetrahedra iso-surface of lattice [Nz,Ny,Nx] fp32 (x fastest) at `level` (csrc/surface.cu; the rule is in
+    include/hg3d.h): count + int64 scans, one device-to-host read of the two totals, emit.
+    -> (vertices [V,3] fp32, normals [V,3] fp32, faces [F,3] int32); empty tensors when nothing crosses."""
+    if lattice.dim() != 3 or lattice.dtype != torch.float32:
+        raise RuntimeError(f"hg3d: iso_surface takes a [Nz,Ny,Nx] fp32 lattice (got {tuple(lattice.shape)} {lattice.dtype})")
+    nz, ny, nx = lattice.shape
+    if min(nz, ny, nx) < 2 or nz * ny * nx > 1 << 30:
+        raise RuntimeError(f"hg3d: iso_surface needs >= 2 points per axis and at most 2^30 points (got {nz} x {ny} x {nx})")
+    level, spacing = float(level), float(spacing)
+    if level != level or not spacing > 0 or len(origin) != 3:
+        raise RuntimeError(f"hg3d: iso_surface needs a finite level, a positive spacing and a 3-d origin "
+                           f"(got level {level}, spacing {spacing}, origin {origin})")
+    dev = lattice.device
+    lat = lattice.contiguous()
+    nbytes = int(lib().hg_iso_workspace_bytes(nz, ny, nx))
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    totals = torch.empty(2, dtype=torch.int64, device=dev)
+    with torch.cuda.device_of(lat):
+        call("hg_iso_count", ptr(lat), nz, ny, nx, level, ptr(ws), nbytes, ptr(totals), stream())
+        V, F = (int(v) for v in totals.cpu())
+        if V >= 1 << 31:
+            raise RuntimeError(f"hg3d: iso_surface found {V} vertices; int32 face indices hold fewer than 2^31")
+        verts = torch.empty(V, 3, dtype=torch.float32, device=dev)
+        normals = torch.empty(V, 3, dtype=torch.float32, device=dev)
+        faces = torch.empty(F, 3, dtype=torch.int32, device=dev)
+        if V:
+            o = [float(v) for v in origin]
+            call("hg_iso_emit", ptr(lat), nz, ny, nx, *o, spacing, level, ptr(ws), nbytes, V, ptr(verts), ptr(normals), ptr(faces),
+                 stream())
+    return verts, normals, faces

@@ -474,6 +474,21 @@ class Map3DGenerator(nn.Module):
             rgb, rgb_render, _ = self._run(freq, phase, styles, conditions, cfg, _precision_passes(kwargs))
         return {"rgbs": rgb, "rgbs_render": rgb_render}
 
+    def truncated_codes(self, latent, truncation_psi, cfg):
+        """latent -> (freq, phase, styles) as `staged_forward` maps them (map3d_generator.py:282-379): the SIREN's codes from
+        the latent or, with neural_field_latent_input False, from a zero latent; truncation_psi < 1 pulls all three towards
+        the averages of `generate_avg_latent` (fresh draws on every call)."""
+        zz = latent if cfg.get("neural_field_latent_input", True) else torch.zeros_like(latent)
+        freq, phase = self.neural_field_mapping_network(zz)
+        _, styles = self.synthesis_mapping_network(latent)
+        if truncation_psi < 1.0:
+            self.generate_avg_latent()
+            _, afreq, aphase, astyles = self.avg_latent
+            freq = afreq + truncation_psi * (freq - afreq)
+            phase = aphase + truncation_psi * (phase - aphase)
+            styles = astyles + truncation_psi * (styles - astyles)
+        return freq, phase, styles
+
     def staged_forward(self, latent, conditions, render_height, render_width, truncation_psi, **kwargs):
         """Inference entry of apps/sample_from_generator.py (map3d_generator.py:282-379): truncation
         towards the average latent, depth map in [-1,1] on the CPU, skeleton passthrough.  The
@@ -482,15 +497,7 @@ class Map3DGenerator(nn.Module):
         with torch.no_grad():
             cfg = self._cfg_for(kwargs, render_height, render_width)
             B = latent.shape[0]
-            zz = latent if cfg.get("neural_field_latent_input", True) else torch.zeros_like(latent)
-            freq, phase = self.neural_field_mapping_network(zz)
-            _, styles = self.synthesis_mapping_network(latent)
-            if truncation_psi < 1.0:
-                self.generate_avg_latent()
-                _, afreq, aphase, astyles = self.avg_latent
-                freq = afreq + truncation_psi * (freq - afreq)
-                phase = aphase + truncation_psi * (phase - aphase)
-                styles = astyles + truncation_psi * (styles - astyles)
+            freq, phase, styles = self.truncated_codes(latent, truncation_psi, cfg)
             rgb, rgb_render, depths = self._run(freq, phase, styles, conditions, cfg, _precision_passes(kwargs))
             focals = conditions["intrinsics"][:, 0, 0]
             scales = conditions["scales"].float()

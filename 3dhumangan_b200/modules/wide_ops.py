@@ -84,13 +84,14 @@ def wide_layer(xs, W512, b512, *, mods=None, act=0, slope=0.2, skips=None, stats
 # ----------------------------------------------------------------------------------------------------------------------
 @torch.no_grad()
 def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix="neural_field.", tape=None, records=None,
-                        sigma_only=False, training=True):
+                        sigma_only=False, point_rgb=False, training=True):
     """-> ray features [B,R,C], rgb [B,R,3] (in [0,1], before the *2-1), depth [B,R,1].
     `tape` (a dict) receives what `render_train.mlp_backward` needs, in the format its docstring describes: per half the
     linear outputs lin_a, lin_b, out_0..3, lin_c, feat, then sig, rgbp and the FiLM tables built from freq / phase
     leaves with autograd history.
     `records` (rec [B,N,36], z_vals [B,N]) replaces the ray stage (hierarchical_sample: the merged samples, with
-    cfg["num_steps"] the samples per ray).  `sigma_only` stops after the sigma head and returns the raw sigma [B,N].
+    cfg["num_steps"] the samples per ray).  `sigma_only` stops after the sigma head and returns the raw sigma [B,N];
+    `point_rgb` stops after the heads and returns the per-point colour [B,N,3] (the sigmoid of the rgb head, before compositing).
     `training` matters with a tape only: `last_back=True` is differentiated for an eval-mode module, refused in train mode."""
     from . import render_train
     abi.require_device()
@@ -187,6 +188,8 @@ def render_forward_wide(P, freq, phase, cond, cfg, u, noise, *, passes=3, prefix
                                     B=B, N=N)
         sig = s_h if sig is None else sig + s_h
         rgbp = r_h if rgbp is None else rgbp + r_h
+    if point_rgb:
+        return torch.sigmoid(rgbp).transpose(1, 2).contiguous()
     nz = None if noise is None else noise.reshape(B, N).float().contiguous()
     comp = dict(B=B, R=R, S=S, noise_std=cfg["nerf_noise"], white_back=cfg.get("white_back", False),
                 softplus=cfg["clamp_mode"] == "softplus", last_back=cfg.get("last_back", False))

@@ -107,6 +107,34 @@ int hg_render_mlp(const float* rec, const float* z_vals, const float* noise, con
                   float* weights_out, float* raw_out, int B, int R, int S, int hidden, float noise_std, int white_back,
                   int last_back, int clamp_softplus, int passes, void* stream);
 
+/* ---- iso-surface of a density lattice (csrc/surface.cu) --------------------------------------------------------------
+ * Marching tetrahedra over the Kuhn split: the cell with lower corner c holds one tet c, c+e_a, c+e_a+e_b, c+(1,1,1) per
+ * axis permutation (a, b, .), taken in the order xyz, xzy, yxz, yzx, zxy, zyx.  The surface is closed and consistently
+ * oriented wherever the level set does not meet the lattice boundary.
+ *   lattice [nz,ny,nx] fp32 (x fastest), every axis >= 2, at most 2^30 points; point (x,y,z) sits at origin + spacing*(x,y,z).
+ *   A value is INSIDE iff it is > level.
+ *   Vertices: point p owns the edges p -> p+d, d in slot order {x, y, z, x+y, x+z, y+z, x+y+z}, that lie in the lattice.  An
+ *     edge whose ends differ in inside-ness gets one vertex: t = (level - v_p) / (v_{p+d} - v_p), position
+ *     origin + spacing * (p + t d); its normal is -grad interpolated as g_p + t (g_{p+d} - g_p) and normalised (zero where
+ *     that is zero), grad by central differences in index units, one-sided at the border.  Every fp32 operation rounds once.
+ *     Vertices are numbered in (point, slot) order.
+ *   Faces: per tet with 1 or 3 inside vertices one triangle on the edges of the lone vertex; with 2 inside (a < b) and 2
+ *     outside (c < d, tet-local order) the quad (ac, ad, bd, bc) split along the diagonal ac-bd into (ac, ad, bd), (ac, bd, bc).
+ *     Winding is counter-clockwise seen from outside (normals point from inside to outside), derived from the parity of the
+ *     tet's axis permutation and of the vertex labelling, never from positions, so degenerate triangles keep it.  Faces are
+ *     numbered in (cell, tet, triangle) order with the cell at its lower corner.
+ * hg_iso_workspace_bytes: device workspace of a lattice (0 for a refused shape).
+ * hg_iso_count: crossing masks, triangle counts and their int64 exclusive scans into the workspace; totals [2] int64 (device) =
+ *               (vertices, faces).
+ * hg_iso_emit : with the workspace of hg_iso_count and n_vertices = totals[0] (< 2^31), writes vertices [V,3], normals [V,3]
+ *               fp32 and faces [F,3] int32.  No atomics decide a position: repeated calls write the same bits. */
+size_t hg_iso_workspace_bytes(int nz, int ny, int nx);
+int hg_iso_count(const float* lattice, int nz, int ny, int nx, float level, void* workspace, size_t workspace_bytes,
+                 long long* totals, void* stream);
+int hg_iso_emit(const float* lattice, int nz, int ny, int nx, float ox, float oy, float oz, float spacing, float level,
+                const void* workspace, size_t workspace_bytes, long long n_vertices, float* vertices, float* normals, int* faces,
+                void* stream);
+
 /* ---- synthesis backbone ---------------------------------------------------------------------- */
 /* Synthesis activations use a tile-blocked planar layout [B, T, C, 128] with T = ceil(Hg*Wg/128): element
  * (b, c, pixel p) lives at ((b*T + p/128)*C + c)*128 + p%128, so the 128 KB a CTA touches per tile are contiguous.
