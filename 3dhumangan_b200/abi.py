@@ -91,6 +91,11 @@ SIGNATURES = {
     "hg_maxpool2x2": (c_int, [c_void_p, c_void_p, c_long, c_int, c_int, c_void_p]),
     "hg_vgg_level_bwd": (c_int, [c_void_p] * 4 + [c_float, c_void_p, c_long, c_int, c_int, c_void_p]),
     "hg_smooth_l1": (c_int, [c_void_p, c_void_p, c_long, c_void_p, c_void_p, c_void_p]),
+    "hg_conv2d_general": (c_int, [c_void_p] + [c_int] * 9 + [c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_int,
+                                                             c_void_p]),
+    "hg_pool3x3": (c_int, [c_void_p] + [c_int] * 7 + [c_void_p, c_int, c_int, c_void_p]),
+    "hg_global_avgpool": (c_int, [c_void_p, c_long, c_int, c_void_p, c_void_p]),
+    "hg_feature_moments": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
     "hg_mt_entry_bytes": (c_int, []),
     "hg_mt_chunk_bytes": (c_int, []),
     "hg_mt_chunk_elems": (c_int, []),

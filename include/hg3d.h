@@ -406,6 +406,24 @@ int hg_vgg_level_bwd(const float* y, const float* t, const float* dpool, const f
                      int H, int W, void* stream);
 int hg_smooth_l1(const float* a, const float* b, long n, float* loss, double* workspace /* >= 2 * #SMs doubles */, void* stream);
 
+/* ---- FID: pytorch-fid's Inception-v3 and the feature statistics (csrc/inception.cu) ------------------------------------------
+ * hg_conv2d_general : out[b, c0 + co, oy, ox] = relu(bias[co] + sum_{ky,kx,ci} W[co,ky,kx,ci] x[b, ci, oy*s - ph + ky,
+ *                     ox*s - pw + kx]) with zero padding, x [B,Cin,H,W], out [B,Ctot,Ho,Wo], Ho = (H + 2 ph - kh) / s + 1 (and
+ *                     Wo likewise); channels of out outside [c0, c0 + Cout) are not touched.  wimg: hg_pack_weight of W
+ *                     [Cout, kh*kw*Cin] with block width Nb <= 128.  kh, kw <= 7, s in {1, 2}, ph < kh, pw < kw, Cout <= 448;
+ *                     passes 3 = bf16x3 (fp32-class), 1 = bf16.
+ * hg_pool3x3        : 3x3 pooling of x [B,C,H,W] into the channel window [c0, c0 + C) of out [B,Ctot,Ho,Wo]: max (avg = 0) at
+ *                     stride 2 / pad 0 or stride 1 / pad 1 (torch's max_pool2d: padding never wins, NaN propagates), average
+ *                     (avg = 1) at stride 1 / pad 1 over the window's in-image elements (count_include_pad=False).
+ * hg_global_avgpool : out[p] = mean of plane p of x [planes, HW].
+ * hg_feature_moments: sum [D] += sum_i f_i and gram [D,D] += sum_i f_i f_i^T in fp64 for features f [n,D] fp32; fixed order,
+ *                     no atomics: repeats are bit-identical. */
+int hg_conv2d_general(const float* x, int B, int Cin, int H, int W, int kh, int kw, int stride, int ph, int pw, const void* wimg,
+                      int Cout, int Nb, const float* bias, float* out, int Ctot, int c0, int passes, void* stream);
+int hg_pool3x3(const float* x, int B, int C, int H, int W, int stride, int pad, int avg, float* out, int Ctot, int c0, void* stream);
+int hg_global_avgpool(const float* x, long planes, int HW, float* out, void* stream);
+int hg_feature_moments(const float* feat, int n, int D, double* sum, double* gram, void* stream);
+
 /* ---- StyleGAN3 native ops named by the reference ---------------------------------------------- */
 /* y = clamp(act(x + b[(i / stepB) % sizeB]) * gain)   replaces bias_act.cpp:32 / bias_act.cu:24 (forward).
  * act: 1 linear 2 relu 3 lrelu 4 tanh 5 sigmoid 6 elu 7 selu 8 softplus 9 swish; clamp < 0 disables. */
