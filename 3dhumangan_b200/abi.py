@@ -96,6 +96,13 @@ SIGNATURES = {
     "hg_pool3x3": (c_int, [c_void_p] + [c_int] * 7 + [c_void_p, c_int, c_int, c_void_p]),
     "hg_global_avgpool": (c_int, [c_void_p, c_long, c_int, c_void_p, c_void_p]),
     "hg_feature_moments": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p, c_void_p]),
+    "hg_row_sqnorms": (c_int, [c_void_p, c_int, c_int, c_void_p, c_void_p]),
+    "hg_knn_radii": (c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p]),
+    "hg_ball_coverage": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p,
+                                 c_void_p, c_void_p]),
+    "hg_kid_workspace_bytes": (c_size_t, [c_int, c_int]),
+    "hg_kid": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t,
+                       c_void_p]),
     "hg_mt_entry_bytes": (c_int, []),
     "hg_mt_chunk_bytes": (c_int, []),
     "hg_mt_chunk_elems": (c_int, []),

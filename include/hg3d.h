@@ -424,6 +424,29 @@ int hg_pool3x3(const float* x, int B, int C, int H, int W, int stride, int pad, 
 int hg_global_avgpool(const float* x, long planes, int HW, float* out, void* stream);
 int hg_feature_moments(const float* feat, int n, int D, double* sum, double* gram, void* stream);
 
+/* ---- KID and k-NN precision / recall on feature sets (csrc/metrics.cu) ------------------------------------------------------
+ * One fp64 pairwise engine (DMMA): every product, sum and comparison is fp64, features x [n,D] are fp32 (widened exactly), no
+ * n x n matrix is written to global memory and no float atomic decides a value, so repeats are bit-identical.  Squared
+ * distances are d^2(a, b) = ||a||^2 + ||b||^2 - 2 a.b clamped at 0, with the norms from hg_row_sqnorms.
+ * hg_row_sqnorms  : out [n] = ||x_i||^2 = x_i . x_i in fp64, on the engine that computes every pairwise product, so two equal
+ *                   rows (in one set or across two) are at d^2 = 0 exactly.
+ * hg_knn_radii    : rho2 [n] = the k-th smallest d^2(x_i, x_j) over j != i (by index: a duplicate row at another index counts
+ *                   at 0); 1 <= k <= 8, k < n.  sqn = hg_row_sqnorms(x).
+ * hg_ball_coverage: row_flag [ng] (bytes) = 1 where some r_j has d^2(g_i, r_j) <= rho2_r[j], col_flag [nr] = 1 where some g_i
+ *                   has d^2(g_i, r_j) <= rho2_g[i], else 0 (col_flag is cleared on the stream first); counts [2] (int64) =
+ *                   (sum row_flag, sum col_flag): precision and recall are counts[0] / ng and counts[1] / nr.
+ * hg_kid          : t [S] fp64, per subset s with rows idx_g[s, :m] of g and idx_r[s, :m] of r (int64, each in range; an
+ *                   index outside it reads as a zero vector): t_s = (sum_{i != j} k(g_i, g_j) + sum_{i != j} k(r_i, r_j)) /
+ *                   (m (m - 1)) - 2 sum_{i,j} k(g_i, r_j) / m^2 with k(a, b) = (a.b / D + 1)^3; the unbiased MMD^2 of KID.
+ *                   2 <= m <= min(ng, nr), S <= 65535; workspace of hg_kid_workspace_bytes(S, m) bytes. */
+int hg_row_sqnorms(const float* x, int n, int D, double* out, void* stream);
+int hg_knn_radii(const float* x, const double* sqn, int n, int D, int k, double* rho2, void* stream);
+int hg_ball_coverage(const float* g, const double* sqn_g, const double* rho2_g, int ng, const float* r, const double* sqn_r,
+                     const double* rho2_r, int nr, int D, unsigned char* row_flag, unsigned char* col_flag, long* counts, void* stream);
+size_t hg_kid_workspace_bytes(int S, int m);
+int hg_kid(const float* g, int ng, const float* r, int nr, int D, const long* idx_g, const long* idx_r, int S, int m, double* t,
+           double* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- StyleGAN3 native ops named by the reference ---------------------------------------------- */
 /* y = clamp(act(x + b[(i / stepB) % sizeB]) * gain)   replaces bias_act.cpp:32 / bias_act.cu:24 (forward).
  * act: 1 linear 2 relu 3 lrelu 4 tanh 5 sigmoid 6 elu 7 selu 8 softplus 9 swish; clamp < 0 disables. */
