@@ -133,7 +133,7 @@ struct CompArgs {
   const float* rgbp;     // [B,3,N]
   const float* feat;     // [B,T,256,128]
   float* ray_out;        // fwd: [B,R,260]
-  float* w_out;          // fwd: [B,N] compositing weights (kept for the backward)
+  float* w_out;          // fwd: [B,N] compositing weights as vr.ray_integration returns them (last_back: absorbed)
   const float* dray;     // bwd: [B,R,260]
   float* dfeat;          // bwd: [B,T,256,128]
   float* drgbp;          // bwd: [B,3,N]
@@ -193,7 +193,7 @@ __global__ void __launch_bounds__(128) composite_kernel(CompArgs a) {
   const float* ft = a.feat + static_cast<long>(tile) * kRC * 128;
 
   if (!kBwd) {
-    a.w_out[gp] = w;
+    a.w_out[gp] = (a.last_back && s == S - 1) ? w + (1.f - rayw[rl]) : w;    // as csrc/render.cu's weights_out
     // weighted sums: warp w handles channels w, w+4, ...; lane l holds points l, l+32, l+64, l+96
     for (int c = warp; c < kRC + 4; c += 4) {
       auto value = [&](int p) {

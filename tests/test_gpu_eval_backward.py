@@ -1,7 +1,7 @@
 """Gradients through the generator in eval() mode: running-statistics BatchNorm, spectral norm from the stored u / v,
-`last_back=True`, a frozen generator differentiated w.r.t. its input alone -- against fp64 torch (the compositing kernel)
-and eval-mode autograd through the oracle (the whole generator; tests/test_oracle_pin_eval_grads.py pins that to the
-reference)."""
+`last_back=True`, a frozen generator differentiated w.r.t. its input alone -- against eval-mode autograd through the
+oracle (the whole generator; tests/test_oracle_pin_eval_grads.py pins that to the reference).  The compositing kernels'
+`last_back` forward and gradient are checked launch by launch in tests/test_gpu_render_kernels.py."""
 import importlib
 
 import pytest
@@ -19,45 +19,7 @@ def _rel(a, b):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
-# 1. hg_render_composite_bwd(last_back=1)
-# ----------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("S", [8, 32, 64])
-@pytest.mark.parametrize("softplus", [False, True])
-@pytest.mark.parametrize("white_back", [False, True])
-def test_composite_backward_last_back(port, S, softplus, white_back):
-    abi = importlib.import_module("3dhumangan_b200.abi")
-    B, R = 2, 256 // S * 3
-    N = R * S
-    g = torch.Generator().manual_seed(S + 2 * softplus + white_back)
-    sig = torch.randn(B, N, generator=g) * 40 + 10         # dense: samples absorb, yet sum w stays below 1 on many rays
-    z = (torch.rand(B, R, S, generator=g) * 0.02 + torch.linspace(0.9, 1.1, S)).sort(-1).values.reshape(B, N)
-    rgbp = torch.randn(B, 3, N, generator=g)
-    feat = torch.randn(B, 256, N, generator=g)
-    dray = torch.randn(B, R, 260, generator=g)
-    dray[..., 259] = 0                                     # depth carries no gradient
-    # fp64 reference: oracle.ray_integration on [feat | sigmoid(rgb) | sigma]
-    sd, fd, rd = sig.double().requires_grad_(True), feat.double().requires_grad_(True), rgbp.double().requires_grad_(True)
-    vals = torch.cat([fd.permute(0, 2, 1), torch.sigmoid(rd).permute(0, 2, 1), sd[..., None]], -1).reshape(B, R, S, 260)
-    out, _, _ = port.ray_integration(vals, z.double().reshape(B, R, S, 1), torch.zeros(B, R, S, 1, dtype=torch.float64), 0.0,
-                                     white_back, True, "softplus" if softplus else "relu")
-    (out * dray[..., :259].double()).sum().backward()
-
-    blocked = lambda t: t.reshape(B, 256, N // 128, 128).permute(0, 2, 1, 3).contiguous().cuda()
-    kw = dict(B=B, R=R, S=S, noise_std=0.0, white_back=white_back, softplus=softplus, last_back=True)
-    ray, _ = abi.render_composite(sig.cuda(), z.cuda(), None, rgbp.cuda(), blocked(feat), **kw)
-    assert (ray[..., :259].cpu().double() - out.detach()).abs().max() < 1e-4 * out.detach().abs().max()
-    df, dp, ds = abi.render_composite_bwd(sig.cuda(), z.cuda(), None, rgbp.cuda(), blocked(feat), dray.cuda(), **kw)
-    torch.cuda.synchronize()
-    df = df.permute(0, 2, 1, 3).reshape(B, 256, N).cpu().double()
-    for got, ref in ((df, fd.grad), (dp.cpu().double(), rd.grad), (ds.cpu().double(), sd.grad)):
-        assert (got - ref).abs().max() < 1e-4 * ref.abs().max()
-    # the flag does something: without it the last sample's gradient differs
-    df0, _, _ = abi.render_composite_bwd(sig.cuda(), z.cuda(), None, rgbp.cuda(), blocked(feat), dray.cuda(), **dict(kw, last_back=False))
-    assert not torch.equal(df0.permute(0, 2, 1, 3).reshape(B, 256, N).cpu().double(), df)
-
-
-# ----------------------------------------------------------------------------------------------------------------------
-# 2.-4. whole generator
+# 1.-3. whole generator
 # ----------------------------------------------------------------------------------------------------------------------
 def _generator(pkg, port, C, mode, legacy, last_back, hier=False, seed=21):
     """An eval-mode generator whose running statistics and u / v come from three train-mode forwards (at random
