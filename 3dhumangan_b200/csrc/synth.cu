@@ -129,8 +129,14 @@ constexpr uint32_t kSynSmemBytes = 2 * kASlots * kAChunk + kSynStages * kBStage 
 constexpr uint32_t kPixSmemBytes = 2 * 3 * kAChunk + kSynStages * kBStage + 3 * kXSlice + (kC * 9 + 512) * 4 + 24 * 8 + 1024;
 static_assert(kSynSmemBytes <= 232448 && kPixSmemBytes <= 232448, "shared memory budget");
 
-// barrier slots
-enum { B_FULL = 0 /*2*/, B_EMPTY = 2 /*2*/, X_FULL = 4 /*5*/, X_EMPTY = 12 /*5*/ };
+// The pixel-style kernel divides the same weight ring into 16 KB units: a [gamma | beta] stage ([128 x 64]) takes one, a
+// conv stage ([256 x 64]) two adjacent ones.
+constexpr int kPixUnits = 4;
+constexpr uint32_t kPixUnit = kBStage / 2;
+static_assert(kPixUnits * kPixUnit == kSynStages * kBStage, "the pixel-style units tile the weight ring");
+
+// barrier slots (const-style uses the first kSynStages of each weight pair, pixel-style all kPixUnits)
+enum { B_FULL = 0 /*4*/, B_EMPTY = 4 /*4*/, X_FULL = 8 /*5*/, X_EMPTY = 13 /*5*/ };
 
 __device__ __forceinline__ void rows_barrier() { named_barrier(1, 256); }
 
@@ -168,7 +174,7 @@ struct TileMap {
 // ------------------------------------------------------------------------------------------
 // common setup
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void init_common(const SpadeArgs& a, const SynSmem& m) {
+__device__ __forceinline__ void init_common(const SpadeArgs& a, const SynSmem& m, int weight_slots) {
   for (int i = threadIdx.x; i < kC; i += blockDim.x) {
     m.tab_bias[i] = a.bias[i];
     m.st_sum[i] = 0.f;
@@ -177,7 +183,7 @@ __device__ __forceinline__ void init_common(const SpadeArgs& a, const SynSmem& m
   if (a.rgb_w)
     for (int i = threadIdx.x; i < 3 * kC; i += blockDim.x) m.tab_rgbw[i] = a.rgb_w[i];
   if (threadIdx.x == 0) {
-    for (int i = 0; i < kSynStages; ++i) {
+    for (int i = 0; i < weight_slots; ++i) {
       mbar_init(m.bars + B_FULL + i, 1);
       mbar_init(m.bars + B_EMPTY + i, 2);             // one arrival per warpgroup
     }
@@ -540,7 +546,7 @@ __global__ void __launch_bounds__(kSynThreads, 1) spade_const_kernel(SpadeArgs a
   extern __shared__ uint8_t smem_raw[];
   const SynSmem m = carve<false>(smem_raw);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  init_common(a, m);
+  init_common(a, m, kSynStages);
   TileMap tm;
   tm.T = (a.HW + 127) / 128;
   tm.first = blockIdx.x;
@@ -669,28 +675,132 @@ __device__ __forceinline__ void bilin(int dst, int in_size, float scale, int& i0
 }
 
 // Weight stages of one pixel-style tile: per conv K chunk kc, the [gamma | beta] rows of channels 64kc.. (128 rows of
-// gamma/beta block kc/2) for both K chunks of A1, then the conv chunk kc.
+// gamma/beta block kc/2) for both K chunks of A1, then the conv chunk kc.  Each 16 KB unit of the ring is filled in turn;
+// a conv stage is two units.  Per K chunk fp32x3 fills 8 units (gb k0 hi / lo, k1 hi / lo, conv hi, conv lo) and bf16 4
+// (gb k0, k1, conv), so a conv stage always starts on unit 0 or 2 and its image is contiguous in shared memory.
 template <int kPasses>
 __device__ __forceinline__ void pixel_weight_producer_loop(const SpadeArgs& a, const SynSmem& m, int num_my_tiles) {
-  uint32_t st = 0, ph = 0;
-  auto emit = [&](const uint8_t* src, uint32_t bytes) {
-    mbar_wait_backoff(m.bars + B_EMPTY + st, ph ^ 1);
-    mbar_arrive_expect_tx(m.bars + B_FULL + st, bytes);
-    bulk_g2s(m.b_st + st * kBStage, src, bytes, m.bars + B_FULL + st);
-    if (++st == kSynStages) { st = 0; ph ^= 1; }
+  uint32_t n = 0;   // units filled
+  auto emit = [&](const uint8_t* src) {
+    const uint32_t u = n % kPixUnits;
+    mbar_wait_backoff(m.bars + B_EMPTY + u, ((n / kPixUnits) & 1) ^ 1);
+    mbar_arrive_expect_tx(m.bars + B_FULL + u, kPixUnit);
+    bulk_g2s(m.b_st + u * kPixUnit, src, kPixUnit, m.bars + B_FULL + u);
+    ++n;
   };
   for (int t = 0; t < num_my_tiles; ++t)
     for (int kc = 0; kc < 4; ++kc) {
       for (int k = 0; k < 2; ++k)
         for (int part = 0; part < (kPasses == 3 ? 2 : 1); ++part)
-          emit(a.wgb + static_cast<size_t>(((kc >> 1) * 2 + k) * 2 + part) * kBStage + (kc & 1) * (kBStage / 2), kBStage / 2);
-      for (int part = 0; part < (kPasses == 3 ? 2 : 1); ++part) emit(a.wimg + static_cast<size_t>(kc * 2 + part) * kBStage, kBStage);
+          emit(a.wgb + static_cast<size_t>(((kc >> 1) * 2 + k) * 2 + part) * kBStage + (kc & 1) * kPixUnit);
+      for (int part = 0; part < (kPasses == 3 ? 2 : 1); ++part) {
+        const uint8_t* src = a.wimg + static_cast<size_t>(kc * 2 + part) * kBStage;
+        emit(src);
+        emit(src + kPixUnit);
+      }
     }
+}
+
+// Consumer side of the unit ring, per warpgroup: a stage of N = 128 takes one unit, N = 256 two.  Like `pipe_chunk`, a
+// stage's units are released (by both warpgroups) once the wgmmas of the NEXT stage have been issued and the stage's own
+// have completed.
+struct PixPipe {
+  uint32_t n = 0;          // units consumed
+  uint32_t prev = 0;       // first unit of the stage awaiting release
+  uint32_t prev_units = 0; // its units (0: none)
+};
+__device__ __forceinline__ void pix_release(const SynSmem& m, PixPipe& p, int t) {
+  if (t == 0)
+    for (uint32_t j = 0; j < p.prev_units; ++j) mbar_arrive(m.bars + B_EMPTY + (p.prev + j) % kPixUnits);
+  p.prev_units = 0;
+}
+// One weight stage (part 0: hi weights, A hi [+ A lo]; part 1: lo weights, A hi) into accumulator d.
+template <int N, int kPasses>
+__device__ __forceinline__ void pix_part(const SynSmem& m, PixPipe& p, float (&d)[N / 2], uint32_t a_hi, uint32_t a_lo, int part,
+                                         bool accumulate, int t) {
+  constexpr uint32_t kUnits = N == 256 ? 2 : 1;
+  const uint32_t u = p.n % kPixUnits;
+#pragma unroll
+  for (uint32_t j = 0; j < kUnits; ++j) mbar_wait(m.bars + B_FULL + u + j, ((p.n + j) / kPixUnits) & 1);
+  acc_fence(d);
+  wgmma_fence();
+  const uint32_t bt = smem_u32(m.b_st + u * kPixUnit);
+  if (part == 0) {
+    wg_k64<N>(d, a_hi, bt, accumulate);
+    if (kPasses == 3) wg_k64<N>(d, a_lo, bt, true);
+  } else {
+    wg_k64<N>(d, a_hi, bt, true);
+  }
+  wgmma_commit();
+  wgmma_wait<1>();
+  acc_fence(d);
+  pix_release(m, p, t);
+  p.prev = u;
+  p.prev_units = kUnits;
+  p.n += kUnits;
+}
+template <int N>
+__device__ __forceinline__ void pix_drain(const SynSmem& m, PixPipe& p, float (&d)[N / 2], int t) {
+  wgmma_wait<0>();
+  acc_fence(d);
+  pix_release(m, p, t);
+}
+
+// A1 = relu(bilinear(P_lr) + c) of tile (b, ti) into the two A1 chunks: column half h builds K chunk h (the previous
+// tile's wgmmas are complete).  Fully unrolled, so that all 64 + 16 loads of a thread are in flight at once: the caller
+// runs it while neither accumulator is live.
+template <int kPasses>
+__device__ __forceinline__ void build_a1(const SpadeArgs& a, const SynSmem& m, int b, int ti, int row, int h, int g, float sy,
+                                         float sx) {
+  const int pix = ti * 128 + row;
+  const bool valid = pix < a.HW;
+  const int py = valid ? pix / a.Wg : 0, px = valid ? pix % a.Wg : 0;
+  int y0, y1, x0, x1;
+  float ly0, ly1, lx0, lx1;
+  bilin(py, a.Rh, sy, y0, y1, ly0, ly1);
+  bilin(px, a.Rw, sx, x0, x1, lx0, lx1);
+  const float* base = a.p_lr + static_cast<long>(b) * a.Rh * a.Rw * a.p_stride;
+  const float4* n00 = reinterpret_cast<const float4*>(base + (static_cast<long>(y0) * a.Rw + x0) * a.p_stride);
+  const float4* n01 = reinterpret_cast<const float4*>(base + (static_cast<long>(y0) * a.Rw + x1) * a.p_stride);
+  const float4* n10 = reinterpret_cast<const float4*>(base + (static_cast<long>(y1) * a.Rw + x0) * a.p_stride);
+  const float4* n11 = reinterpret_cast<const float4*>(base + (static_cast<long>(y1) * a.Rw + x1) * a.p_stride);
+  const float4* pb = a.p_bias ? reinterpret_cast<const float4*>(a.p_bias + static_cast<long>(b) * 128) : nullptr;
+  const float2 lx0p = make_float2(lx0, lx0), lx1p = make_float2(lx1, lx1), ly0p = make_float2(ly0, ly0), ly1p = make_float2(ly1, ly1);
+#pragma unroll
+  for (int gi = 0; gi < 8; ++gi) {
+    float y[8];
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      const int f4 = h * 16 + gi * 2 + u;
+      const float4 v00 = __ldg(n00 + f4), v01 = __ldg(n01 + f4), v10 = __ldg(n10 + f4), v11 = __ldg(n11 + f4);
+      // same association as upsample_bilinear2d: ly0*(lx0*a + lx1*b) + ly1*(lx0*c + lx1*d), on channel pairs
+      auto lerp2 = [&](float2 a, float2 b, float2 c, float2 d) {
+        const float2 top = ffma2(b, lx1p, fmul2(a, lx0p));
+        const float2 bot = ffma2(d, lx1p, fmul2(c, lx0p));
+        return ffma2(top, ly0p, fmul2(bot, ly1p));
+      };
+      float2 lo2 = lerp2(make_float2(v00.x, v00.y), make_float2(v01.x, v01.y), make_float2(v10.x, v10.y), make_float2(v11.x, v11.y));
+      float2 hi2 = lerp2(make_float2(v00.z, v00.w), make_float2(v01.z, v01.w), make_float2(v10.z, v10.w), make_float2(v11.z, v11.w));
+      if (pb) {
+        const float4 c4 = __ldg(pb + f4);
+        lo2 = fadd2(lo2, make_float2(c4.x, c4.y));
+        hi2 = fadd2(hi2, make_float2(c4.z, c4.w));
+      }
+      y[u * 4 + 0] = lo2.x; y[u * 4 + 1] = lo2.y; y[u * 4 + 2] = hi2.x; y[u * 4 + 3] = hi2.y;
+    }
+#pragma unroll
+    for (int j = 0; j < 8; ++j) y[j] = valid ? fmaxf(y[j], 0.f) : 0.f;
+    store_a8<kPasses == 3>(m.a_hi + h * kAChunk, m.a_lo + h * kAChunk, row, gi * 8, y);
+  }
+  fence_proxy_async_smem();
+  named_barrier(2 + g, 128);
 }
 
 // Per tile: A1 = relu(bilinear(P_lr) + c) (K = 128, two chunks); then per conv K chunk kc: [gamma | beta] of channels
 // 64kc.. = A1 . Wgb (a [64 x 128] accumulator per warpgroup), y = lrelu(BN(x)*(1+gamma)+beta) -> the y chunk, conv
 // accumulate.  The 28x larger up-sampled style map of map3d_generator.py:244-245 is never materialised.
+// The A1 gather and the epilogue run with the tensor pipe idle, but while the weight producer refills the ring for the
+// next tile; DESIGN.md section 8 item 1 records what moving them under the wgmmas measured.
 template <int kPasses>
 __global__ void __launch_bounds__(kSynThreads, 1) spade_pixel_kernel(SpadeArgs a) {
   extern __shared__ uint8_t smem_raw[];
@@ -701,7 +811,7 @@ __global__ void __launch_bounds__(kSynThreads, 1) spade_pixel_kernel(SpadeArgs a
     m.tab_g0[i] = a.scsh[kC + i];
   }
   for (int i = threadIdx.x; i < 512; i += blockDim.x) m.tab_bgb[i] = a.bgb[i];
-  init_common(a, m);
+  init_common(a, m, kPixUnits);
   TileMap tm;
   tm.T = (a.HW + 127) / 128;
   tm.first = blockIdx.x;
@@ -717,57 +827,21 @@ __global__ void __launch_bounds__(kSynThreads, 1) spade_pixel_kernel(SpadeArgs a
     const int row = q * 32 + lane;
     uint8_t* const y_hi = m.a_hi + 2 * kAChunk;
     uint8_t* const y_lo = m.a_lo + 2 * kAChunk;
+    constexpr int kParts = kPasses == 3 ? 2 : 1;
     uint32_t xg = 0, sg = 0;
-    Pipe p;
+    PixPipe p;
     float d[128], e[64];
     for (int it = 0; it < tm.count; ++it) {
       int b, ti;
       tm.get(it, b, ti);
-      const int pix = ti * 128 + row;
-      const bool valid = pix < a.HW;
-      // ---- A1 = relu(bilinear(P_lr) + c): column half h builds K chunk h (the previous tile's wgmmas are complete)
-      {
-        const int py = valid ? pix / a.Wg : 0, px = valid ? pix % a.Wg : 0;
-        int y0, y1, x0, x1;
-        float ly0, ly1, lx0, lx1;
-        bilin(py, a.Rh, sy, y0, y1, ly0, ly1);
-        bilin(px, a.Rw, sx, x0, x1, lx0, lx1);
-        const float* base = a.p_lr + static_cast<long>(b) * a.Rh * a.Rw * a.p_stride;
-        const float4* n00 = reinterpret_cast<const float4*>(base + (static_cast<long>(y0) * a.Rw + x0) * a.p_stride);
-        const float4* n01 = reinterpret_cast<const float4*>(base + (static_cast<long>(y0) * a.Rw + x1) * a.p_stride);
-        const float4* n10 = reinterpret_cast<const float4*>(base + (static_cast<long>(y1) * a.Rw + x0) * a.p_stride);
-        const float4* n11 = reinterpret_cast<const float4*>(base + (static_cast<long>(y1) * a.Rw + x1) * a.p_stride);
-        const float4* pb = a.p_bias ? reinterpret_cast<const float4*>(a.p_bias + static_cast<long>(b) * 128) : nullptr;
-        const float2 lx0p = make_float2(lx0, lx0), lx1p = make_float2(lx1, lx1), ly0p = make_float2(ly0, ly0), ly1p = make_float2(ly1, ly1);
-#pragma unroll 2
-        for (int gi = 0; gi < 8; ++gi) {
-          float y[8];
+      build_a1<kPasses>(a, m, b, ti, row, h, g, sy, sx);
+      // The first wgmma into each accumulator in a tile runs with scale-d = 0 and ignores its input; defining both here
+      // tells the compiler so (the wgmma operands are read-write), and frees their 192 registers for the epilogue and
+      // the A1 gather above.  Without it the gather could only run 2 iterations deep, and the kernel spilled.
 #pragma unroll
-          for (int u = 0; u < 2; ++u) {
-            const int f4 = h * 16 + gi * 2 + u;
-            const float4 v00 = __ldg(n00 + f4), v01 = __ldg(n01 + f4), v10 = __ldg(n10 + f4), v11 = __ldg(n11 + f4);
-            // same association as upsample_bilinear2d: ly0*(lx0*a + lx1*b) + ly1*(lx0*c + lx1*d), on channel pairs
-            auto lerp2 = [&](float2 a, float2 b, float2 c, float2 d) {
-              const float2 top = ffma2(b, lx1p, fmul2(a, lx0p));
-              const float2 bot = ffma2(d, lx1p, fmul2(c, lx0p));
-              return ffma2(top, ly0p, fmul2(bot, ly1p));
-            };
-            float2 lo2 = lerp2(make_float2(v00.x, v00.y), make_float2(v01.x, v01.y), make_float2(v10.x, v10.y), make_float2(v11.x, v11.y));
-            float2 hi2 = lerp2(make_float2(v00.z, v00.w), make_float2(v01.z, v01.w), make_float2(v10.z, v10.w), make_float2(v11.z, v11.w));
-            if (pb) {
-              const float4 c4 = __ldg(pb + f4);
-              lo2 = fadd2(lo2, make_float2(c4.x, c4.y));
-              hi2 = fadd2(hi2, make_float2(c4.z, c4.w));
-            }
-            y[u * 4 + 0] = lo2.x; y[u * 4 + 1] = lo2.y; y[u * 4 + 2] = hi2.x; y[u * 4 + 3] = hi2.y;
-          }
+      for (int i = 0; i < 128; ++i) d[i] = 0.f;
 #pragma unroll
-          for (int j = 0; j < 8; ++j) y[j] = valid ? fmaxf(y[j], 0.f) : 0.f;
-          store_a8<kPasses == 3>(m.a_hi + h * kAChunk, m.a_lo + h * kAChunk, row, gi * 8, y);
-        }
-        fence_proxy_async_smem();
-        named_barrier(2 + g, 128);
-      }
+      for (int i = 0; i < 64; ++i) e[i] = 0.f;
       int frow[2];
       bool fvalid[2];
 #pragma unroll
@@ -778,10 +852,13 @@ __global__ void __launch_bounds__(kSynThreads, 1) spade_pixel_kernel(SpadeArgs a
 #pragma unroll 1
       for (int kc = 0; kc < 4; ++kc) {
         // ---- [gamma | beta] of channels 64kc.. (waits for the previous conv chunk too: the y chunk is free afterwards)
-        for (int k = 0; k < 2; ++k)
-          pipe_chunk<128, kPasses>(m, p, e, smem_u32(m.a_hi + k * kAChunk) + g * 64 * 128, smem_u32(m.a_lo + k * kAChunk) + g * 64 * 128,
-                                   k > 0, t);
-        pipe_drain<128>(m, p, e, t);
+#pragma unroll
+        for (int s = 0; s < 2 * kParts; ++s) {
+          const int k = s / kParts;
+          pix_part<128, kPasses>(m, p, e, smem_u32(m.a_hi + k * kAChunk) + g * 64 * 128, smem_u32(m.a_lo + k * kAChunk) + g * 64 * 128,
+                                 s % kParts, s > 0, t);
+        }
+        pix_drain<128>(m, p, e, t);
         // ---- y = lrelu(BN(x)*(1+gamma)+beta) straight from the fragments; x from the chunk's two activation slices
         const uint32_t s0 = ring_take(m, xg, 0, m.xs_n), s1 = ring_take(m, xg + 1, 0, m.xs_n);
         xg += 2;
@@ -814,9 +891,11 @@ __global__ void __launch_bounds__(kSynThreads, 1) spade_pixel_kernel(SpadeArgs a
         ring_release(m, s1);
         fence_proxy_async_smem();
         named_barrier(2 + g, 128);
-        pipe_chunk<256, kPasses>(m, p, d, smem_u32(y_hi) + g * 64 * 128, smem_u32(y_lo) + g * 64 * 128, kc > 0, t);
+#pragma unroll
+        for (int part = 0; part < kParts; ++part)
+          pix_part<256, kPasses>(m, p, d, smem_u32(y_hi) + g * 64 * 128, smem_u32(y_lo) + g * 64 * 128, part, kc > 0, t);
       }
-      pipe_drain<256>(m, p, d, t);
+      pix_drain<256>(m, p, d, t);
       epilogue_fwd_any(a, m, d, b, ti, tm.T, g, t, sg);
     }
     flush_fwd_stats(a, m);
