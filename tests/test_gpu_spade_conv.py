@@ -15,86 +15,21 @@ Shapes derive from the device's SM count: a one-tile image, last tiles with fewe
 pixels (warpgroup 1 holds only padding in the first two), and a launch whose persistent CTAs each walk tiles of several
 samples (per-sample table refresh; backward: per-sample flush of the sums)."""
 import importlib
-import itertools
-import math
 
 import pytest
 import torch
 import torch.nn.functional as F
 
+from blocked_util import (C, SHAPES, U, _blocked, _check_stats, _guarded, _intact, _nsm, _pairwise, _planar, _shape, _tiles,
+                          _tiles_per_cta)
+
 pytestmark = pytest.mark.gpu
 
-C = 256
 STAT_STRIDE = 520          # modules/synthesis_ops.py: [0:256] sum, [256:512] sumsq, [512] count, pad
-U = 2.0 ** -24             # fp32 unit roundoff
-G = 64                     # guard elements on each side of an output (keeps 16-byte alignment in fp32 and fp64)
-SENTINEL = -1234.5
 
 
 def _abi():
     return importlib.import_module("3dhumangan_b200.abi")
-
-
-def _nsm():
-    return torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
-
-
-SHAPES = ["tile1", "lt64", "eq64", "gt64", "multi"]
-
-
-def _shape(name):
-    """(B, Hg, Wg) of a named case."""
-    if name == "tile1":
-        return 2, 8, 12            # HW 96: one tile per sample
-    if name == "lt64":
-        return 2, 12, 26           # HW 312: last tile holds 56 valid pixels
-    if name == "eq64":
-        return 2, 16, 20           # HW 320: last tile holds exactly 64
-    if name == "gt64":
-        return 2, 40, 25           # HW 1000: last tile holds 104
-    n = _nsm()                     # "multi": T < SMs tiles per sample and B*T >= 2 SMs tiles
-    Wg = 100
-    Hg = (n // 3 + 1) * 128 // Wg
-    T = (Hg * Wg + 127) // 128
-    B = -(-2 * n // T) + 1
-    assert T < n and B * T >= 2 * n and (Hg * Wg) % 128
-    return B, Hg, Wg
-
-
-def _tiles(HW):
-    return (HW + 127) // 128
-
-
-def _tiles_per_cta(B, HW):
-    tiles = B * _tiles(HW)
-    return -(-tiles // min(tiles, _nsm()))
-
-
-def _blocked(t, fill=0.0):
-    """[B,C,HW] -> tile-blocked [B,T,C,128]; the rows past the image hold `fill`."""
-    B, Cc, HW = t.shape
-    T = _tiles(HW)
-    pad = torch.full((B, Cc, T * 128), fill, dtype=t.dtype, device=t.device)
-    pad[:, :, :HW] = t
-    return pad.reshape(B, Cc, T, 128).permute(0, 2, 1, 3).contiguous()
-
-
-def _planar(t, HW):
-    B, T, Cc, _ = t.shape
-    return t.permute(0, 2, 1, 3).reshape(B, Cc, T * 128)[:, :, :HW]
-
-
-def _guarded(shape, dtype=torch.float32, fill=float("nan")):
-    """(buffer, view): a contiguous view of `shape` inside a buffer with G sentinel elements on each side."""
-    n = math.prod(shape)
-    buf = torch.full((n + 2 * G,), SENTINEL, dtype=dtype, device="cuda")
-    view = buf[G:G + n].view(shape)
-    view.fill_(fill)
-    return buf, view
-
-
-def _intact(buf):
-    return bool((buf[:G] == SENTINEL).all()) and bool((buf[-G:] == SENTINEL).all())
 
 
 def _stats_row(count):
@@ -118,21 +53,6 @@ def _rel_max(got, ref):
 
 def _lrelu(v, slope):
     return torch.where(v > 0, v, slope * v)
-
-
-def _pairwise(levels):
-    """Rows of the full product of `levels` (a dict name -> values) chosen greedily until every pair of values of every two
-    options appears in some row; deterministic."""
-    names = list(levels)
-    todo = {(a, va, b, vb) for a, b in itertools.combinations(names, 2) for va in levels[a] for vb in levels[b]}
-    rows = []
-    while todo:
-        best = max(itertools.product(*levels.values()),
-                   key=lambda r: sum((a, r[i], b, r[j]) in todo for (i, a), (j, b) in itertools.combinations(enumerate(names), 2)))
-        d = dict(zip(names, best))
-        todo -= {(a, d[a], b, d[b]) for a, b in itertools.combinations(names, 2)}
-        rows.append(d)
-    return rows
 
 
 def _vid(v):
@@ -163,21 +83,6 @@ def _render_size(ratio, Hg, Wg):
 # ----------------------------------------------------------------------------------------------------------------------
 # shared checks
 # ----------------------------------------------------------------------------------------------------------------------
-def _check_stats(row, init, outp, n_t):
-    """row = init + (sum, sumsq) over the valid pixels of the kernel's own out, per channel, in fp64.
-    Bound: per tile and channel a thread adds its 2 rows (1 fp32 add), three shuffle steps fold the 16 rows of a warp
-    (3 adds), and each of the 8 warps adds its total to the CTA's fp32 shared sum, over n_t tiles per CTA: at most
-    4 + 8 n_t roundings on any path, each at most u = 2^-24 of a partial sum bounded by sum |v| (sumsq: sum v^2), so
-    |err| <= (4 + 8 n_t) u sum|v| (first-order gamma_n bound).  The CTA sums then go to the fp64 row (2^-53 per add)."""
-    o = outp.double()
-    terms = ((o.sum((0, 2)), o.abs().sum((0, 2))), ((o * o).sum((0, 2)), (o * o).sum((0, 2))))
-    for k, (ref, mag) in enumerate(terms):
-        err = (row[k * C:(k + 1) * C] - init[k * C:(k + 1) * C] - ref).abs()
-        bound = (4 + 8 * n_t) * U * mag + 1e-13 * init[k * C:(k + 1) * C].abs()
-        assert (err <= bound).all(), ("sum" if k == 0 else "sumsq", float((err / bound).max()))
-    assert torch.equal(row[512:], init[512:]), "the count and pad slots [512:520] must stay untouched"
-
-
 def _check_rgb(rgb_out, outp, rgb_w, rgb_b, rgb_in):
     """rgb_out = W_rgb out + b (+ rgb_in) in fp64 from the kernel's own out.  Per pixel a lane runs 64 sequential fp32
     fmas (its 64 channels), two shuffle adds fold the 4 lanes of a row, then b and rgb_in are added: at most 68

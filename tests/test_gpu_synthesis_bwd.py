@@ -1,5 +1,6 @@
-"""Backward kernels of the const-style SPADE half-block (csrc/synth.cu kBwd, csrc/synth_bwd.cu) against the
-same gradients written with plain torch ops in fp64 (autograd through SPADE2d/SPADEBlock, map3d_layers.py:176-238)."""
+"""The synthesis network's backward (modules/synthesis_train.py::synthesis_backward) against fp64 autograd through the
+restated reference (SPADE2d/SPADEBlock, map3d_layers.py:176-238).  Its kernels are tested launch by launch in
+tests/test_gpu_synthesis_bwd_kernels.py."""
 import importlib
 
 import pytest
@@ -10,128 +11,9 @@ pytestmark = pytest.mark.gpu
 C = 256
 
 
-def _blocked(t, fill=0.0):
-    """[B,C,HW] -> tile-blocked [B,T,C,128]; the rows past the image hold `fill` (zero; NaN = what an uninitialised
-    activation buffer may hold there in production: nothing may leak from them)."""
-    B, Cc, HW = t.shape
-    T = (HW + 127) // 128
-    pad = torch.full((B, Cc, T * 128), fill, dtype=t.dtype, device=t.device)
-    pad[:, :, :HW] = t
-    return pad.reshape(B, Cc, T, 128).permute(0, 2, 1, 3).contiguous()
-
-
 def _planar(t, HW):
     B, T, Cc, _ = t.shape
     return t.permute(0, 2, 1, 3).reshape(B, Cc, T * 128)[:, :, :HW]
-
-
-def _case(B, Hg, Wg, seed):
-    g = torch.Generator().manual_seed(seed)
-    HW = Hg * Wg
-    x = torch.randn(B, C, HW, generator=g)
-    dout = torch.randn(B, C, HW, generator=g)
-    mod = torch.stack([1.0 + 0.5 * torch.randn(B, C, generator=g), 0.5 * torch.randn(B, C, generator=g)], dim=1)   # [B,2,C]
-    W = torch.randn(C, C, generator=g) / 16
-    return x, dout, mod, W
-
-
-@pytest.mark.parametrize("B,Hg,Wg", [(2, 24, 20), (3, 32, 32)])
-@pytest.mark.parametrize("passes,tol", [(3, 2e-5), (1, 2e-2)])
-def test_dgrad(B, Hg, Wg, passes, tol):
-    abi = importlib.import_module("3dhumangan_b200.abi")
-    x, dout, mod, W = _case(B, Hg, Wg, 1)
-    HW = Hg * Wg
-    xd, dd = x.double(), dout.double()
-    pre = xd * mod[:, 0, :, None].double() + mod[:, 1, :, None].double()
-    dy = torch.einsum("oc,bop->bcp", W.double(), dd)
-    dpre_ref = dy * torch.where(pre > 0, 1.0, 0.2)
-    s1_ref, s2_ref = dpre_ref.sum(2), (dpre_ref * xd).sum(2)
-
-    wimg_t, _ = abi.pack_weight(W.t().contiguous().cuda(), Nb=256)
-    xb, db_ = _blocked(x, float("nan")).cuda(), _blocked(dout, float("nan")).cuda()
-    dpre = torch.full_like(xb, float("nan"))
-    sums = torch.zeros(B, 2, C, dtype=torch.float64, device="cuda")
-    T = xb.shape[1]
-    abi.spade_bwd_dgrad(db_, xb, T * C * 128, mod.cuda().contiguous(), wimg_t, dpre, sums, B=B, Hg=Hg, Wg=Wg, passes=passes)
-    torch.cuda.synchronize()
-    got = _planar(dpre, HW).cpu().double()
-    # pre-activations within rounding distance of zero may legitimately pick the other slope
-    safe = pre.abs() > 1e-5
-    err = ((got - dpre_ref) * safe).abs().max() / dpre_ref.abs().max()
-    assert err < tol, err
-    assert (sums[:, 0].cpu() - s1_ref).abs().max() / s1_ref.abs().max() < 10 * tol
-    assert (sums[:, 1].cpu() - s2_ref).abs().max() / s2_ref.abs().max() < 10 * tol
-
-
-def test_dgrad_shared_input():
-    """x with batch stride 0 (the synthesis input is shared by the batch)."""
-    abi = importlib.import_module("3dhumangan_b200.abi")
-    B, Hg, Wg = 2, 16, 24
-    x, dout, mod, W = _case(B, Hg, Wg, 2)
-    x = x[:1]
-    HW = Hg * Wg
-    pre = x.double() * mod[:, 0, :, None].double() + mod[:, 1, :, None].double()
-    ref = torch.einsum("oc,bop->bcp", W.double(), dout.double()) * torch.where(pre > 0, 1.0, 0.2)
-    wimg_t, _ = abi.pack_weight(W.t().contiguous().cuda(), Nb=256)
-    dpre = torch.empty(B, (HW + 127) // 128, C, 128, device="cuda")
-    sums = torch.zeros(B, 2, C, dtype=torch.float64, device="cuda")
-    abi.spade_bwd_dgrad(_blocked(dout).cuda(), _blocked(x).cuda()[0], 0, mod.cuda().contiguous(), wimg_t, dpre, sums, B=B, Hg=Hg, Wg=Wg)
-    got = _planar(dpre, HW).cpu().double()
-    assert ((got - ref) * (pre.abs() > 1e-5)).abs().max() / ref.abs().max() < 2e-5
-
-
-@pytest.mark.parametrize("B,Hg,Wg", [(2, 24, 20), (3, 64, 48)])
-@pytest.mark.parametrize("passes,tol", [(3, 2e-5), (1, 2e-2)])
-def test_wgrad(B, Hg, Wg, passes, tol):
-    abi = importlib.import_module("3dhumangan_b200.abi")
-    x, dout, mod, _ = _case(B, Hg, Wg, 3)
-    pre = x.double() * mod[:, 0, :, None].double() + mod[:, 1, :, None].double()
-    y = torch.where(pre > 0, pre, 0.2 * pre)
-    dw_ref = torch.einsum("bop,bcp->oc", dout.double(), y)
-    db_ref = dout.double().sum((0, 2))
-    xb = _blocked(x, float("nan")).cuda()
-    dw, db = abi.spade_bwd_wgrad(_blocked(dout, float("nan")).cuda(), xb, xb.shape[1] * C * 128, mod.cuda().contiguous(), B=B, Hg=Hg,
-                                 Wg=Wg, passes=passes)
-    torch.cuda.synchronize()
-    assert (dw.cpu().double() - dw_ref).abs().max() / dw_ref.abs().max() < tol
-    assert (db.cpu().double() - db_ref).abs().max() / db_ref.abs().max() < 1e-5
-
-
-@pytest.mark.parametrize("with_rgb,with_skip,with_dpre", [(True, True, True), (False, False, True), (True, False, False),
-                                                          (False, True, True)])
-def test_combine(with_rgb, with_skip, with_dpre):
-    abi = importlib.import_module("3dhumangan_b200.abi")
-    B, Hg, Wg = 2, 20, 18          # HW = 360: last tile partial, multiple of 4
-    HW = Hg * Wg
-    g = torch.Generator().manual_seed(4)
-    x = torch.randn(B, C, HW, generator=g)
-    dpre = torch.randn(B, C, HW, generator=g)
-    dskip = torch.randn(B, C, HW, generator=g)
-    drgb = torch.randn(B, 3, HW, generator=g)
-    rgb_w = torch.randn(3, C, generator=g)
-    g1 = torch.randn(B, 2, C, generator=g)
-    ak = torch.randn(2, C, generator=g)
-    ref = torch.zeros(B, C, HW, dtype=torch.float64)
-    if with_dpre:
-        ref += dpre.double() * g1[:, 0, :, None].double() + ak[0, None, :, None].double() + ak[1, None, :, None].double() * x.double()
-    if with_skip:
-        ref += dskip.double()
-    if with_rgb:
-        ref += torch.einsum("jc,bjp->bcp", rgb_w.double(), drgb.double())
-    dw_ref = torch.einsum("bjp,bcp->jc", drgb.double(), x.double())
-    xb = _blocked(x).cuda()
-    dx = torch.full_like(xb, float("nan"))
-    dwrgb = torch.zeros(3, C, dtype=torch.float64, device="cuda")
-    abi.spade_bwd_combine(dx, B=B, Hg=Hg, Wg=Wg, dpre=_blocked(dpre).cuda() if with_dpre else None, x=xb,
-                          x_bstride=xb.shape[1] * C * 128, g1=g1.cuda() if with_dpre else None, ak=ak.cuda() if with_dpre else None,
-                          dskip=_blocked(dskip).cuda() if with_skip else None, drgb=drgb.cuda() if with_rgb else None,
-                          rgb_w=rgb_w.cuda() if with_rgb else None, dwrgb=dwrgb if with_rgb else None)
-    torch.cuda.synchronize()
-    assert torch.isfinite(dx).all()
-    assert (dx[:, -1, :, HW % 128:] == 0).all()          # padding pixels of the last tile stay zero
-    assert (_planar(dx, HW).cpu().double() - ref).abs().max() < 1e-4
-    if with_rgb:
-        assert (dwrgb.cpu() - dw_ref).abs().max() / dw_ref.abs().max() < 1e-5
 
 
 def _network_case(port, monkeypatch, mod_blocks, mode, Rh, Rw, seed, C=C):
