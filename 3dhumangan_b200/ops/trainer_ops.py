@@ -240,6 +240,10 @@ class FusedAdam(torch.optim.Optimizer):
             shadow = {id(p): s for p, s in zip(req, ema.shadow_params)}
             if any(id(p) not in shadow for _, p in flat if p.requires_grad):
                 raise RuntimeError("hg3d: the EMA does not cover this optimiser's parameters")
+        # refuse before any state changes: a refused call must leave `step` (and so every later bias correction) as it was
+        pairs = {(gi, int(self.state[p]["step"]) + 1 if len(self.state[p]) else 1) for gi, p in flat if p.grad is not None}
+        if len(pairs) > 8:
+            raise RuntimeError("hg3d: FusedAdam handles at most 8 distinct (group, step) pairs per call")
         # per-(group, step) scalars
         sgroups, sidx = [], {}
         ents = np.zeros((len(flat), 6), dtype=np.int64)
@@ -278,8 +282,7 @@ class FusedAdam(torch.optim.Optimizer):
                 chunk_rows.append((ti, sg, off))
         if not sgroups:
             sgroups.append((0.0, 0.0, 0.0, 1.0, 0.0, 1.0, 1.0))          # nothing to step; the EMA (if any) still runs
-        if len(sgroups) > 8:
-            raise RuntimeError("hg3d: FusedAdam handles at most 8 distinct (group, step) pairs per call")
+        assert len(sgroups) == max(1, len(pairs))
         assert int(abi.lib().hg_mt_entry_bytes()) == 48 and int(abi.lib().hg_mt_chunk_bytes()) == 16
         table = torch.from_numpy(ents).to(dev, non_blocking=True)
         ch = np.zeros((len(chunk_rows), 2), dtype=np.int64)

@@ -81,14 +81,23 @@ def _intact(buf):
     return bool((buf[:G] == SENTINEL).all()) and bool((buf[-G:] == SENTINEL).all())
 
 
-def _pairwise(levels):
-    """Rows of the full product of `levels` (a dict name -> values) chosen greedily until every pair of values of every two
-    options appears in some row; deterministic."""
+def _pairs(levels, valid=None):
+    """Every (option, value, option, value) pair that some row of the product of `levels` allowed by `valid` contains."""
     names = list(levels)
-    todo = {(a, va, b, vb) for a, b in itertools.combinations(names, 2) for va in levels[a] for vb in levels[b]}
+    rows = [dict(zip(names, r)) for r in itertools.product(*levels.values())]
+    return {(a, d[a], b, d[b]) for d in rows if valid is None or valid(d) for a, b in itertools.combinations(names, 2)}
+
+
+def _pairwise(levels, valid=None):
+    """Rows of the full product of `levels` (a dict name -> values), restricted to the rows `valid` accepts (all when None),
+    chosen greedily until every pair of values of every two options that some allowed row holds appears in a row;
+    deterministic."""
+    names = list(levels)
+    todo = _pairs(levels, valid)
+    cands = [r for r in itertools.product(*levels.values()) if valid is None or valid(dict(zip(names, r)))]
     rows = []
     while todo:
-        best = max(itertools.product(*levels.values()),
+        best = max(cands,
                    key=lambda r: sum((a, r[i], b, r[j]) in todo for (i, a), (j, b) in itertools.combinations(enumerate(names), 2)))
         d = dict(zip(names, best))
         todo -= {(a, d[a], b, d[b]) for a, b in itertools.combinations(names, 2)}
