@@ -103,6 +103,9 @@ SIGNATURES = {
     "hg_kid_workspace_bytes": (c_size_t, [c_int, c_int]),
     "hg_kid": (c_int, [c_void_p, c_int, c_void_p, c_int, c_int, c_void_p, c_void_p, c_int, c_int, c_void_p, c_void_p, c_size_t,
                        c_void_p]),
+    "hg_lpips_workspace_bytes": (c_size_t, [c_int]),
+    "hg_lpips_level": (c_int, [c_void_p, c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_void_p, c_size_t, c_void_p]),
+    "hg_lpips_input": (c_int, [c_void_p, c_int, c_int, c_int, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
     "hg_mt_entry_bytes": (c_int, []),
     "hg_mt_chunk_bytes": (c_int, []),
     "hg_mt_chunk_elems": (c_int, []),

@@ -71,6 +71,7 @@ class VGG16Features(torch.nn.Module):
         self.register_buffer("mean", torch.tensor(MEAN), persistent=False)
         self.register_buffer("std", torch.tensor(STD), persistent=False)
         self._packed = None
+        self._packed_convs = None
         if weights is None or isinstance(weights, (str, os.PathLike)):
             path = default_weights_path() if weights is None else os.fspath(weights)
             if not os.path.isfile(path):
@@ -93,13 +94,23 @@ class VGG16Features(torch.nn.Module):
     def _convs(self):
         return list(self._modules["features"].children())
 
+    def conv_images(self):
+        """Per convolution (img, Nb), packed again only when a convolution weight changed.  `ppl.LPIPS` reads these too, so
+        an LPIPS on this network never packs fc6 / fc7."""
+        convs = self._convs()
+        key = tuple((c.weight.data_ptr(), c.weight._version, str(c.weight.device)) for c in convs)
+        if self._packed_convs is None or self._packed_convs[0] != key:
+            with torch.no_grad():
+                self._packed_convs = (key, [_pack(c.weight.float()) for c in convs])
+        return self._packed_convs[1]
+
     def _images(self):
         """(per convolution (img, Nb), per fc layer [(c0, Cout, img, Nb, bias)]), packed again only when a weight changed."""
-        convs, fcs = self._convs(), [self.classifier._modules["0"], self.classifier._modules["3"]]
-        key = tuple((p.data_ptr(), p._version, str(p.device)) for p in self.parameters())
+        fcs = [self.classifier._modules["0"], self.classifier._modules["3"]]
+        conv_imgs = self.conv_images()
+        key = tuple((p.data_ptr(), p._version, str(p.device)) for layer in fcs for p in layer.parameters())
         if self._packed is None or self._packed[0] != key:
             with torch.no_grad():
-                conv_imgs = [_pack(c.weight.float()) for c in convs]
                 fc6 = fcs[0].weight.float().view(DIM, 512, 7, 7).permute(0, 2, 3, 1).reshape(DIM, -1)
                 fc_imgs = []
                 for w, layer in ((fc6, fcs[0]), (fcs[1].weight.float(), fcs[1])):
@@ -110,8 +121,8 @@ class VGG16Features(torch.nn.Module):
                         img, Nb = abi.pack_weight(w[c0:c0 + cout].contiguous(), Nb=-(-cout // (16 * nblocks)) * 16)
                         wins.append((c0, cout, img, Nb, layer.bias[c0:c0 + cout].float().contiguous()))
                     fc_imgs.append(wins)
-            self._packed = (key, (conv_imgs, fc_imgs))
-        return self._packed[1]
+            self._packed = (key, fc_imgs)
+        return conv_imgs, self._packed[1]
 
     def _check(self, images):
         abi.require_device()

@@ -474,16 +474,20 @@ class Map3DGenerator(nn.Module):
             rgb, rgb_render, _ = self._run(freq, phase, styles, conditions, cfg, _precision_passes(kwargs))
         return {"rgbs": rgb, "rgbs_render": rgb_render}
 
-    def truncated_codes(self, latent, truncation_psi, cfg):
+    def truncated_codes(self, latent, truncation_psi, cfg, averages=None):
         """latent -> (freq, phase, styles) as `staged_forward` maps them (map3d_generator.py:282-379): the SIREN's codes from
         the latent or, with neural_field_latent_input False, from a zero latent; truncation_psi < 1 pulls all three towards
-        the averages of `generate_avg_latent` (fresh draws on every call)."""
+        the averages of `generate_avg_latent` (fresh draws on every call), or towards `averages` = (freq, phase, styles)
+        when they are given."""
         zz = latent if cfg.get("neural_field_latent_input", True) else torch.zeros_like(latent)
         freq, phase = self.neural_field_mapping_network(zz)
         _, styles = self.synthesis_mapping_network(latent)
         if truncation_psi < 1.0:
-            self.generate_avg_latent()
-            _, afreq, aphase, astyles = self.avg_latent
+            if averages is None:
+                self.generate_avg_latent()
+                _, afreq, aphase, astyles = self.avg_latent
+            else:
+                afreq, aphase, astyles = averages
             freq = afreq + truncation_psi * (freq - afreq)
             phase = aphase + truncation_psi * (phase - aphase)
             styles = astyles + truncation_psi * (styles - astyles)

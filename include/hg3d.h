@@ -447,6 +447,19 @@ size_t hg_kid_workspace_bytes(int S, int m);
 int hg_kid(const float* g, int ng, const float* r, int nr, int D, const long* idx_g, const long* idx_r, int S, int m, double* t,
            double* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- Perceptual path length: LPIPS (VGG, v0.1) heads and the PPL input stage (csrc/ppl.cu) ---------------------------------
+ * hg_lpips_input : out [B,3,H/f,W/f] = (mean of x [B,3,H,W] over each f x f window - shift[c]) / scale[c]; H and W divisible by
+ *                  f (else refused).  shift / scale [3] on the device.
+ * hg_lpips_level : acc [B] fp64 += (1 / HW) sum_p sum_c w[c] (a[b,c,p] / (|a[b,:,p]| + 1e-10) - b'[b,c,p] / (|b'[b,:,p]| + 1e-10))^2
+ *                  for the features a = f0, b' = f1 [B,C,HW] fp32 of the two endpoints of B pairs and the lin weights w [C];
+ *                  norms, differences and sums in fp64, in a fixed order without atomics (repeats are bit-identical, and a
+ *                  pair's value does not depend on the other pairs).  C <= 1024, B <= 65535; workspace of
+ *                  hg_lpips_workspace_bytes(B) bytes. */
+size_t hg_lpips_workspace_bytes(int B);
+int hg_lpips_level(const float* f0, const float* f1, const float* w, int B, int C, int HW, double* acc, double* workspace,
+                   size_t workspace_bytes, void* stream);
+int hg_lpips_input(const float* x, int B, int H, int W, int f, const float* shift, const float* scale, float* out, void* stream);
+
 /* ---- StyleGAN3 native ops named by the reference ---------------------------------------------- */
 /* y = clamp(act(x + b[(i / stepB) % sizeB]) * gain)   replaces bias_act.cpp:32 / bias_act.cu:24 (forward).
  * act: 1 linear 2 relu 3 lrelu 4 tanh 5 sigmoid 6 elu 7 selu 8 softplus 9 swish; clamp < 0 disables. */

@@ -4,13 +4,18 @@
     python tools/evaluate.py gen   --config 420|tiny [--checkpoint generator.pth] --num N --out gen_feats.npz [--batch 8]
                                    [--seed 0] [--truncation 1.0] [--inception PATH] [--vgg PATH]
     python tools/evaluate.py score real_feats.npz gen_feats.npz [--subsets 100] [--subset-size 1000] [--k 3]
+    python tools/evaluate.py ppl   --config 420|tiny [--checkpoint generator.pth] [--num 50000] [--batch 8] [--seed 0]
+                                   [--space w|z] [--sampling end|full] [--epsilon 1e-4] [--truncation 1.0] [--vgg PATH]
+                                   [--lpips PATH]
 
 `real` reads the image folder under the rules of `tools/fid.py real` (every PNG / JPEG at its stored size) and `gen` samples
 the generator as `tools/fid.py gen` does (same seeds, same ray-jitter seeding, torchrun-capable, rank 0 writes).  Both write
 one .npz with the Inception pool features (`inception`, [N,2048]) and the VGG16 fc7 features (`vgg16`, [N,4096]) of every
 image, so all metrics come from one pass over the images.  `score` prints one JSON line with `fid`, `kid`, `kid_std`,
-`precision`, `recall`, `n_real`, `n_gen`, `k`, `subsets` and `subset_size`.  The detectors' weights default to the cached
-pytorch-fid and torchvision files, which are never downloaded."""
+`precision`, `recall`, `n_real`, `n_gen`, `k`, `subsets` and `subset_size`.  `ppl` prints one JSON line with the perceptual
+path length of the generator (`3dhumangan_b200.ppl.path_length`; torchrun-capable like `gen`, rank 0 prints): `ppl`, `lo`,
+`hi`, `num`, `batch`, `seed`, `space`, `sampling`, `epsilon` and `truncation`.  The detectors' weights default to the cached
+pytorch-fid and torchvision files, and LPIPS's lin weights to `ppl.default_lin_path()`; none is ever downloaded."""
 import argparse
 import importlib
 import json
@@ -85,6 +90,28 @@ def gen(args):
         dist.destroy_process_group()
 
 
+def ppl(args):
+    import torch.distributed as dist
+    from invert import released_like
+    pkg = importlib.import_module("3dhumangan_b200")
+    metrics = importlib.import_module("3dhumangan_b200.metrics")
+    ppl_mod = importlib.import_module("3dhumangan_b200.ppl")
+    if "RANK" in os.environ and not dist.is_initialized():
+        torch.cuda.set_device(int(os.environ.get("LOCAL_RANK", 0)))
+        dist.init_process_group("nccl")
+    G, cfg, _ = released_like(pkg, args.config, args.checkpoint)
+    G.set_device(torch.device("cuda", torch.cuda.current_device()))
+    lpips = ppl_mod.LPIPS(vgg=metrics.VGG16Features(weights=args.vgg), lin=args.lpips).cuda()
+    res = ppl_mod.path_length(G, cfg, args.num, args.batch, seed=args.seed, space=args.space, sampling=args.sampling,
+                              epsilon=args.epsilon, truncation_psi=args.truncation, lpips=lpips)
+    if not dist.is_initialized() or dist.get_rank() == 0:
+        print(json.dumps({"ppl": res["ppl"], "lo": res["lo"], "hi": res["hi"], "num": args.num, "batch": args.batch,
+                          "seed": args.seed, "space": args.space, "sampling": args.sampling, "epsilon": args.epsilon,
+                          "truncation": args.truncation}))
+    if dist.is_initialized():
+        dist.destroy_process_group()
+
+
 def score(args):
     fid, metrics = _mods()
     r, g = metrics.load_features(args.real), metrics.load_features(args.gen)
@@ -126,6 +153,18 @@ def parser():
     s.add_argument("--subsets", type=int, default=100)
     s.add_argument("--subset-size", type=int, default=1000)
     s.add_argument("--k", type=int, default=3)
+    p = sub.add_parser("ppl")
+    p.add_argument("--config", choices=["420", "tiny"], default="420")
+    p.add_argument("--checkpoint")
+    p.add_argument("--num", type=int, default=50000)
+    p.add_argument("--batch", type=int, default=8)
+    p.add_argument("--seed", type=int, default=0)
+    p.add_argument("--space", choices=["w", "z"], default="w")
+    p.add_argument("--sampling", choices=["end", "full"], default="end")
+    p.add_argument("--epsilon", type=float, default=1e-4)
+    p.add_argument("--truncation", type=float, default=1.0)
+    p.add_argument("--vgg")
+    p.add_argument("--lpips")
     return ap
 
 
@@ -133,7 +172,7 @@ def main(argv=None):
     args = parser().parse_args(argv)
     if not torch.cuda.is_available():
         raise SystemExit(f"evaluate {args.cmd}: needs a CUDA device")
-    {"real": real, "gen": gen, "score": score}[args.cmd](args)
+    {"real": real, "gen": gen, "score": score, "ppl": ppl}[args.cmd](args)
 
 
 if __name__ == "__main__":
