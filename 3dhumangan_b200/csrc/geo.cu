@@ -287,8 +287,9 @@ __global__ void __launch_bounds__(kGeoThreads, 1) geo_kernel(GeoArgs a) {
       a.points[gp * 3 + 2] = pz;
     }
 
-    // K=1 nearest posed vertex (smpl.py:220), exact oracle arithmetic
-    float best = 3.4e38f;
+    // K=1 nearest posed vertex (smpl.py:220), exact oracle arithmetic.  best starts at +inf so that a d2 which
+    // overflows to inf is still a candidate (lowest index on the tie); only a NaN d2 is never taken.
+    float best = INFINITY;
     int bi = 0x7fffffff;
     auto consider = [&](const float4 q) {
       const float ex = __fsub_rn(px, q.x), ey = __fsub_rn(py, q.y), ez = __fsub_rn(pz, q.z);
@@ -334,6 +335,9 @@ __global__ void __launch_bounds__(kGeoThreads, 1) geo_kernel(GeoArgs a) {
         }
       }
     }
+    // a NaN point took no candidate: index 0 and d2 NaN, as knn_points' min / first-argmin gives, and never a row
+    // index from the sentinel below
+    if (bi == 0x7fffffff) { bi = 0; best = __int_as_float(0x7fffffff); }
     if (a.nearest) a.nearest[gp] = bi;
     if (a.nearest_d2) a.nearest_d2[gp] = best;
 

@@ -152,12 +152,18 @@ __global__ void __launch_bounds__(kSampleWarps * 32) merge_samples_kernel(
   int* src = s_src[warp];
   for (int e = lane; e < n; e += 32) zs[e] = e < S ? fine_z[ray * S + e] : coarse_z[ray * S + e - S];
   __syncwarp();
+  // rank in the total order of torch.sort: every number before NaN, equal keys (NaN with NaN included) by position.
+  // The ranks are then a permutation of [0, n) for any input, so every slot of src is written exactly once.
   for (int e = lane; e < n; e += 32) {
     const float v = zs[e];
+    const bool vnan = isnan(v);
     int rank = 0;
     for (int k = 0; k < n; ++k) {
       const float w = zs[k];
-      rank += (w < v) || (w == v && k < e);
+      const bool wnan = isnan(w);
+      const bool less = vnan ? !wnan : (w < v);
+      const bool same = vnan ? wnan : (w == v);
+      rank += less || (same && k < e);
     }
     src[rank] = e;
   }
