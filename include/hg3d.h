@@ -201,7 +201,9 @@ int hg_conv1x1_blocked(const float* x, int Cin, const void* wimg, const float* b
                        int passes, void* stream);
 /* act (0 LeakyReLU/ReLU, 1 sine/cosine) selects the mask; ascale scales the operand per (sample, channel) before the
  * product: [B,256] over g, or with g2 [B,512] (columns 0..255 scale g, 256..511 scale g2); rk_* adds  sum_j rk_w[j][c]*rk_v[b][j][pixel]  (rk_w [3,256], rk_v [B,rk_n,HW], rk_n in 1..3) to the
- * product before the mask -- the sigma / rgb heads of the renderer (modulated.py:62-73) feed back that way. */
+ * product before the mask -- the sigma / rgb heads of the renderer (modulated.py:62-73) feed back that way.  rk_w is
+ * read as a full [3,256] table whatever rk_n is (rows past rk_n are multiplied by zero), so those rows must be finite;
+ * rk_v is read only in its first rk_n rows per sample. */
 int hg_conv1x1_blocked_bwd(const float* g, const float* g2, const float* aux, const float* mod, const void* wimg_t,
                            float* out, double* sums, int Cout, float slope, int pixel_major, int act, const float* ascale,
                            const float* rk_w, const float* rk_v, int rk_n, int B, int Hg, int Wg, int passes,

@@ -603,12 +603,15 @@ def test_render_heads_bwd(shape):
 # ----------------------------------------------------------------------------------------------------------------------
 # 5. hg_act_wgrad_blocked
 # ----------------------------------------------------------------------------------------------------------------------
-WGRAD = {   # name -> (act, Cx, pscale, shape)
-    "sine-pscale-few": (1, 256, True, "few"),
-    "sine-pscale-multi": (1, 256, True, "multi"),
-    "sine-nopscale-multi": (1, 256, False, "multi"),
-    "identity-cx128-few": (2, 128, True, "few"),
-    "identity-cx128-multi": (2, 128, True, "multi"),
+WGRAD = {   # name -> (act, Cx, pscale, shape, passes); passes 1 is the bf16 training leg (hg_precision="bf16")
+    "sine-pscale-few": (1, 256, True, "few", 3),
+    "sine-pscale-multi": (1, 256, True, "multi", 3),
+    "sine-nopscale-multi": (1, 256, False, "multi", 3),
+    "identity-cx128-few": (2, 128, True, "few", 3),
+    "identity-cx128-multi": (2, 128, True, "multi", 3),
+    "sine-pscale-multi-p1": (1, 256, True, "multi", 1),
+    "sine-nopscale-multi-p1": (1, 256, False, "multi", 1),
+    "identity-cx128-multi-p1": (2, 128, True, "multi", 1),
 }
 
 
@@ -634,10 +637,13 @@ def test_act_wgrad_blocked(case):
     Bound: bf16x3 operands drop at most 3 * 2^-18 of each product (48 U), one rounding of ps*dout, fp32 accumulation of
     64-term chunks and of the 6 n_t chunk products a CTA adds, then a fixed-order fp64 reduction:
     |err| <= (116 + 6 n_t) U sum |terms| + sum |ps dout| (|t| U + SIN_ABS for the sine; |t| U for the affine).
-    Measured on an H100 80GB HBM3 (700 W): at most 0.18 of the bound; one tile scaled with another image's pscale row
-    fails by 277x or more."""
+    One bf16 pass (passes 1) rounds each operand once to 8 significant bits, so a product carries up to 2^-8 + 2^-18
+    (64 U) in place of the 48 U of bf16x3: |err| <= 2^-8 sum |terms| + (132 + 6 n_t) U sum |terms| + the same sine term.
+    That worst-case bound is ~500x the bf16x3 one and cannot see a one-tile fault, so the fault runs at passes 3 only.
+    Measured on an H100 80GB HBM3 (700 W): at most 0.18 of the bound (0.025 at passes 1); one tile scaled with another
+    image's pscale row fails by 277x or more."""
     abi = _abi()
-    act, Cx, use_ps, shape = WGRAD[case]
+    act, Cx, use_ps, shape, passes = WGRAD[case]
     B, Hg, Wg = _wgrad_shape(shape)
     HW = Hg * Wg
     T = -(-HW // 128)
@@ -668,7 +674,7 @@ def test_act_wgrad_blocked(case):
         b2, db = _guarded((C,))
         db_, xb = blocked(dout, fill), blocked(x, fill)
         abi.call("hg_act_wgrad_blocked", abi.ptr(db_), abi.ptr(ps), abi.ptr(xb), T * Cx * 128, Cx, abi.ptr(mod), act, abi.ptr(dw),
-                 abi.ptr(db), abi.ptr(ws), B, C, Hg, Wg, 3, abi.stream())
+                 abi.ptr(db), abi.ptr(ws), B, C, Hg, Wg, passes, abi.stream())
         torch.cuda.synchronize()      # the workspace is shared by the launches
         return dw.clone(), db.clone(), (b1, b2)
     runs = [launch(float("nan")), launch(0.0), launch(0.0)]
@@ -688,7 +694,8 @@ def test_act_wgrad_blocked(case):
         gd = dout.double() * (psd[:, :, None] if psd is not None else 1.0)
         ref_w = torch.einsum("bop,bip->oi", gd, y)
         ref_b = gd.sum((0, 2))
-        bw = (116 + 6 * n_t) * U * torch.einsum("bop,bip->oi", gd.abs(), y.abs()) + torch.einsum("bop,bip->oi", gd.abs(), ey)
+        coef = (116 + 6 * n_t) * U if passes == 3 else 2.0 ** -8 + (132 + 6 * n_t) * U
+        bw = coef * torch.einsum("bop,bip->oi", gd.abs(), y.abs()) + torch.einsum("bop,bip->oi", gd.abs(), ey)
         bb = (116 + 6 * n_t) * U * gd.abs().sum((0, 2))
         return ref_w, ref_b, bw, bb
     psd = ps.double() if ps is not None else None
@@ -697,7 +704,7 @@ def test_act_wgrad_blocked(case):
     chk.add("dW", (dw.double() - ref_w).abs(), bw)
     chk.add("db", (db.double() - ref_b).abs(), bb)
     chk.done()
-    if ps is not None and B > 1:
+    if ps is not None and B > 1 and passes == 3:
         # one tile's pscale row belonging to the wrong image: tile 0 of image 1 scaled with image 0's row
         x_t = x[1:2, :, :128]
         gd_t = dout[1:2, :, :128].double()
