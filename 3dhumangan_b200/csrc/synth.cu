@@ -10,8 +10,10 @@
 // Per CTA (384 threads), persistent over tiles of 128 pixels of one image: warpgroup g (warps 4g..4g+3) builds the bf16
 // hi/lo operand rows of pixels 64g..64g+63 (BN, SPADE modulation, LeakyReLU fused), issues their wgmmas ([64 x 256] fp32
 // accumulator in registers) and runs the epilogue (bias, residual, ToRGB, next-BatchNorm statistics, plane stores); warps
-// 8, 9, 10 each stream one ring with cp.async.bulk (weights, activation slices, residual slices: one producer per ring,
-// since a single producer couples the rings by program order and deadlocks).
+// 8 and 9 stream the weights and the staging slices with cp.async.bulk.  The const-style forward's staging ring carries
+// each tile's activation slices, then its residual slices, in the order the warpgroups take them, so the residual of an
+// epilogue loads up to 5 slices ahead; the backward and the pixel-style kernel keep a separate residual ring streamed by
+// warp 10 (one producer per ring, since a single producer of two rings couples them by program order and deadlocks).
 //
 // Two variants:
 //   const-style : gamma/beta are per-sample vectors (blocks whose style map is spatially constant, 12 of 18
@@ -39,9 +41,8 @@ constexpr int kC = 256;             // channels (hidden_dim == feature_dim == 25
 constexpr int kSynThreads = 384;
 constexpr int kSynStages = 2;       // weight stages
 constexpr int kASlots = 2;          // operand ring
-constexpr int kXSlots = 5;          // staging slots in total
-constexpr int kXs = 3;              //   slots 0..2: activation slices (operand team)
-constexpr int kSs = 2;              //   slots 3..4: residual slices (epilogue team)
+constexpr int kXSlots = 5;          // const-style staging slots in total: forward, one ring of activation slices, each
+                                    // tile's followed by its residual slices; backward, 3 activation + 2 residual slots
 constexpr uint32_t kAChunk = 128 * 128;   // [128 x 64] bf16
 constexpr uint32_t kBStage = 256 * 128;   // [256 x 64] bf16
 constexpr uint32_t kXSlice = 32 * 128 * 4;  // 32 channels x 128 pixels fp32
@@ -88,7 +89,8 @@ struct SynSmem {
   uint8_t* a_lo;
   uint8_t* b_st;
   float* x_st;     // staging slots [32][128]: activation ring, then residual ring
-  int xs_n, ss_n;  // slots of the two rings
+  int xs_n, ss_n;  // slots of the activation ring (0..xs_n-1) and of the residual ring after it; ss_n = 0: the residual
+                   // slices follow each tile's activation slices through the activation ring
   float* tab_g1;   // [C]  (const: g1 | pixel: bn scale)
   float* tab_g0;   // [C]  (const: g0 | pixel: bn shift)
   float* tab_bias; // [C]
@@ -100,8 +102,9 @@ struct SynSmem {
   uint64_t* bars;
 };
 
-// const-style: 2 operand slots, 3 + 2 staging slots; pixel-style: 3 operand chunks, 2 + 1 staging slots
-template <bool kPixel>
+// const-style: 2 operand slots, one 5-slot staging ring (kOneRing) or 3 + 2 staging slots; pixel-style: 3 operand chunks,
+// 2 + 1 staging slots
+template <bool kPixel, bool kOneRing = false>
 __device__ __forceinline__ SynSmem carve(uint8_t* raw) {
   constexpr int kA = kPixel ? 3 : kASlots, kX = kPixel ? 3 : kXSlots;
   uint8_t* s = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(raw) + 1023) & ~uintptr_t(1023));
@@ -110,8 +113,8 @@ __device__ __forceinline__ SynSmem carve(uint8_t* raw) {
   m.a_lo = s + kA * kAChunk;
   m.b_st = s + 2 * kA * kAChunk;
   m.x_st = reinterpret_cast<float*>(m.b_st + kSynStages * kBStage);
-  m.xs_n = kPixel ? 2 : kXs;
-  m.ss_n = kPixel ? 1 : kSs;
+  m.xs_n = kPixel ? 2 : kOneRing ? kXSlots : 3;
+  m.ss_n = kPixel ? 1 : kOneRing ? 0 : 2;
   float* f = m.x_st + kX * (kXSlice / 4);
   m.tab_g1 = f; f += kC;
   m.tab_g0 = f; f += kC;
@@ -139,6 +142,37 @@ static_assert(kPixUnits * kPixUnit == kSynStages * kBStage, "the pixel-style uni
 enum { B_FULL = 0 /*4*/, B_EMPTY = 4 /*4*/, X_FULL = 8 /*5*/, X_EMPTY = 13 /*5*/ };
 
 __device__ __forceinline__ void rows_barrier() { named_barrier(1, 256); }
+
+// Phase profile of the const-style forward, off by default: built with -DHG_SPADE_PROFILE, thread 0 of each MMA warpgroup
+// sums %globaltimer intervals per phase over its walk and adds them to g_spade_prof (read and cleared by
+// hg_spade_profile_read; slot kProfPhases counts warpgroup-tiles).  Without the macro every HG_PROF_* expands to nothing.
+#ifdef HG_SPADE_PROFILE
+enum { PROF_XRING, PROF_BUILD, PROF_WRING, PROF_MMA, PROF_DRAIN, PROF_EPI, PROF_TABLE, kProfPhases };
+__device__ unsigned long long g_spade_prof[kProfPhases + 1];
+__device__ __forceinline__ uint64_t prof_now() {
+  uint64_t v;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(v));
+  return v;
+}
+#define HG_PROF_BEGIN uint64_t prof_t = prof_now(), prof_acc[kProfPhases + 1] = {}
+#define HG_PROF(k)                      \
+  do {                                  \
+    const uint64_t prof_n = prof_now(); \
+    prof_acc[k] += prof_n - prof_t;     \
+    prof_t = prof_n;                    \
+  } while (0)
+#define HG_PROF_TILE ++prof_acc[kProfPhases]
+#define HG_PROF_END(t)                                                                          \
+  do {                                                                                          \
+    if ((t) == 0)                                                                               \
+      for (int k = 0; k <= kProfPhases; ++k) atomicAdd(&g_spade_prof[k], static_cast<unsigned long long>(prof_acc[k])); \
+  } while (0)
+#else
+#define HG_PROF_BEGIN
+#define HG_PROF(k)
+#define HG_PROF_TILE
+#define HG_PROF_END(t)
+#endif
 
 __device__ __forceinline__ float lrelu02(float v) { return v > 0.f ? v : 0.2f * v; }
 
@@ -250,7 +284,8 @@ __device__ __forceinline__ void pipe_drain(const SynSmem& m, Pipe& p, float (&d)
 }
 
 // ------------------------------------------------------------------------------------------
-// warp 9: activation slices, warp 10: residual slices: two independent rings.
+// warp 9: activation slices (const-style forward: followed by each tile's residual slices in the same ring), warp 10:
+// residual slices in a ring of their own (backward, pixel-style).
 // ------------------------------------------------------------------------------------------
 __device__ __forceinline__ void ring_emit(const SynSmem& m, uint32_t& g, int base, int slots, const float* src) {
   const uint32_t slot = base + g % slots;
@@ -269,10 +304,14 @@ __device__ __forceinline__ void x_producer_loop(const SpadeArgs& a, const SynSme
     const float* base2 = a.x2 ? a.x2 + (static_cast<long>(b) * tm.T + ti) * a.xC * 128 : nullptr;
     for (int j = 0; j < 2 * a.nkc; ++j)
       ring_emit(m, g, 0, m.xs_n, (j < per_src ? base : base2 - per_src * 32 * 128) + j * 32 * 128);
+    if (m.ss_n == 0 && a.skip) {   // one ring: the residual slices the epilogue takes after this tile's operand
+      const float* sbase = a.skip + static_cast<long>(b) * a.skip_bstride + static_cast<long>(ti) * a.cout * 128;
+      for (int j = 0; j < a.cout / 32; ++j) ring_emit(m, g, 0, m.xs_n, sbase + j * 32 * 128);
+    }
   }
 }
 __device__ __forceinline__ void skip_producer_loop(const SpadeArgs& a, const SynSmem& m, const TileMap& tm) {
-  if (!a.skip) return;
+  if (!a.skip || m.ss_n == 0) return;
   uint32_t g = 0;
   for (int it = 0; it < tm.count; ++it) {
     int b, ti;
@@ -314,7 +353,8 @@ __device__ __forceinline__ void take_x_pair(const SynSmem& m, uint32_t& xg, int 
 // r = (t%32)/4.  A transposing reduction over r (lane bits 2..4: each step keeps half of the values and adds the partner's
 // copy of the same half) leaves lane r the total of value k = r, i.e. column 8 (r/2) + 2 (t%4) + r%2: 7 shuffles and one
 // warp-wide shared atomic instead of 24 shuffles and 8 atomics from 4 lanes (a float atomic on shared memory is a
-// compare-and-swap loop, so every atomic instruction is a serial retry loop).
+// compare-and-swap loop, so every atomic instruction is a serial retry loop).  The atomic is issued on the shared
+// window explicitly: through a generic pointer it compiles to a run-time dispatch over global and shared atomics.
 __device__ __forceinline__ void column_sums(float* st, int c0, const float (&v)[4][2]) {
   const int lane = threadIdx.x & 31, r = lane >> 2;
   const bool b2 = r & 4, b1 = r & 2, b0 = r & 1;
@@ -328,7 +368,8 @@ __device__ __forceinline__ void column_sums(float* st, int c0, const float (&v)[
   for (int i = 0; i < 2; ++i)     // k = i + 2 b1 + 4 b2
     u[i] = (b1 ? w[i + 2] : w[i]) + __shfl_xor_sync(0xffffffffu, b1 ? w[i] : w[i + 2], 8);
   const float x = (b0 ? u[1] : u[0]) + __shfl_xor_sync(0xffffffffu, b0 ? u[0] : u[1], 4);   // k = r
-  atomicAdd(st + c0 + 8 * (r >> 1) + 2 * (lane & 3) + (r & 1), x);
+  asm volatile("red.shared.add.f32 [%0], %1;" ::"r"(smem_u32(st + c0 + 8 * (r >> 1) + 2 * (lane & 3) + (r & 1))), "f"(x)
+               : "memory");
 }
 
 // ------------------------------------------------------------------------------------------
@@ -349,19 +390,24 @@ __device__ __forceinline__ void epilogue_fwd(const SpadeArgs& a, const SynSmem& 
   }
   float* const otile = a.out + (static_cast<long>(b) * T + ti) * cout * 128;
   float r[2][3] = {{0.f, 0.f, 0.f}, {0.f, 0.f, 0.f}};
+  // tables and slices are read through the shared window (LDS): through the generic pointers of SynSmem every read is a
+  // generic load.  The tables are fixed after init_common.
+  uint32_t tbias = smem_u32(m.tab_bias), trgbw = smem_u32(m.tab_rgbw);
+  opaque(tbias);
+  opaque(trgbw);
 #pragma unroll
   for (int cg = 0; cg < 8; ++cg) {
     if (cg * 32 >= cout) break;
     float sk[2][4][2];
     if (kSkip) {
-      const uint32_t slot = ring_take(m, sg, m.xs_n, m.ss_n);
-      const float* xs = m.x_st + slot * (kXSlice / 4);
+      const uint32_t slot = m.ss_n ? ring_take(m, sg, m.xs_n, m.ss_n) : ring_take(m, sg, 0, m.xs_n);
+      const uint32_t xs = smem_u32(m.x_st + slot * (kXSlice / 4));
 #pragma unroll
       for (int i = 0; i < 2; ++i)
 #pragma unroll
         for (int jj = 0; jj < 4; ++jj)
 #pragma unroll
-          for (int e = 0; e < 2; ++e) sk[i][jj][e] = xs[(frag_col(t, jj, e)) * 128 + row[i]];
+          for (int e = 0; e < 2; ++e) sk[i][jj][e] = lds_f32(xs + ((frag_col(t, jj, e)) * 128 + row[i]) * 4);
       ring_release(m, slot);
       ++sg;
     }
@@ -371,7 +417,12 @@ __device__ __forceinline__ void epilogue_fwd(const SpadeArgs& a, const SynSmem& 
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
         const int j = cg * 4 + jj, c = frag_col(t, j, e);
-        const float bc = m.tab_bias[c];
+        const float bc = lds1(tbias + c * 4);
+        float wk[3];
+        if (kRgb) {
+#pragma unroll
+          for (int k = 0; k < 3; ++k) wk[k] = lds1(trgbw + (k * kC + c) * 4);
+        }
         s1[jj][e] = 0.f;
         s2[jj][e] = 0.f;
 #pragma unroll
@@ -382,7 +433,7 @@ __device__ __forceinline__ void epilogue_fwd(const SpadeArgs& a, const SynSmem& 
           else v = 0.f;
           if (kRgb) {
 #pragma unroll
-            for (int k = 0; k < 3; ++k) r[i][k] = fmaf(v, m.tab_rgbw[k * kC + c], r[i][k]);
+            for (int k = 0; k < 3; ++k) r[i][k] = fmaf(v, wk[k], r[i][k]);
           }
           s1[jj][e] += v;
           s2[jj][e] = fmaf(v, v, s2[jj][e]);
@@ -537,14 +588,15 @@ __device__ __forceinline__ void flush_bwd_sums(const SpadeArgs& a, const SynSmem
 // ------------------------------------------------------------------------------------------
 // const-style variant (384 threads).  Warpgroup g (warps 4g..4g+3) builds rows 64g..64g+63 of each K chunk in a 2-slot
 // ring (warp (q, h): rows 32q.., channels 32h.. of the chunk), issues their wgmmas ([64 x 256] fp32 accumulator in
-// registers) and runs the epilogue; warp 8 streams the weights, warp 9 the activation slices, warp 10 the residual slices.
+// registers) and runs the epilogue; warp 8 streams the weights, warp 9 the activation slices (forward: and behind each
+// tile's, its residual slices, through one 5-slot ring), warp 10 the backward's residual slices.
 // kBwd: data gradient of the same half-block: the operand is dL/dout passed through unchanged (optionally scaled), the
 // weight image is W^T, the epilogue is `epilogue_bwd`.
 // ------------------------------------------------------------------------------------------
 template <int kPasses, bool kBwd>
 __global__ void __launch_bounds__(kSynThreads, 1) spade_const_kernel(SpadeArgs a) {
   extern __shared__ uint8_t smem_raw[];
-  const SynSmem m = carve<false>(smem_raw);
+  const SynSmem m = carve<false, !kBwd>(smem_raw);   // the backward's epilogue spills with the single ring
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   init_common(a, m, kSynStages);
   TileMap tm;
@@ -560,12 +612,15 @@ __global__ void __launch_bounds__(kSynThreads, 1) spade_const_kernel(SpadeArgs a
     const int row = q * 32 + lane;
     int cur_b = -1;
     uint32_t acnt = 0;   // operand chunks produced (2-slot ring)
-    uint32_t xg = 0, sg = 0;
+    uint32_t xg = 0, sg = 0;   // slices taken from the activation ring (forward: and the residual slices behind them)
+                               // and from the backward's residual ring
     Pipe p;
     float d[128];
+    HG_PROF_BEGIN;
     for (int it = 0; it < tm.count; ++it) {
       int b, ti;
       tm.get(it, b, ti);
+      HG_PROF_TILE;
       if (b != cur_b) {  // refresh the per-sample tables (and, backward, flush the previous sample's sums)
         rows_barrier();
         if (kBwd && cur_b >= 0) flush_bwd_sums(a, m, cur_b);
@@ -608,7 +663,9 @@ __global__ void __launch_bounds__(kSynThreads, 1) spade_const_kernel(SpadeArgs a
         const bool second = two_tables && kc * 64 >= kC;
         const uint32_t tg1 = second ? tg1b : tg1a, tg0 = second ? tg0b : tg0a;
         float cur[32];
+        HG_PROF(PROF_TABLE);
         take_x_pair(m, xg, h, row, cur);
+        HG_PROF(PROF_XRING);
         // the slot was last read by chunk acnt - 2, whose wgmmas pipe_chunk has seen complete
         const uint32_t slot = acnt & 1;
 #pragma unroll
@@ -638,13 +695,22 @@ __global__ void __launch_bounds__(kSynThreads, 1) spade_const_kernel(SpadeArgs a
         }
         fence_proxy_async_smem();
         named_barrier(2 + g, 128);
+        HG_PROF(PROF_BUILD);
+#ifdef HG_SPADE_PROFILE
+        mbar_wait(m.bars + B_FULL + p.st, p.ph);   // pipe_chunk's first wait then returns at once
+        HG_PROF(PROF_WRING);
+#endif
         pipe_chunk<256, kPasses>(m, p, d, smem_u32(m.a_hi + slot * kAChunk) + g * 64 * 128,
                                  smem_u32(m.a_lo + slot * kAChunk) + g * 64 * 128, kc > 0, t);
+        HG_PROF(PROF_MMA);
       }
       pipe_drain<256>(m, p, d, t);
+      HG_PROF(PROF_DRAIN);
       if (kBwd) epilogue_bwd_any(a, m, d, b, ti, tm.T, g, t, sg);
-      else epilogue_fwd_any(a, m, d, b, ti, tm.T, g, t, sg);
+      else epilogue_fwd_any(a, m, d, b, ti, tm.T, g, t, xg);
+      HG_PROF(PROF_EPI);
     }
+    HG_PROF_END(t);
     if (kBwd) {
       rows_barrier();
       if (cur_b >= 0) flush_bwd_sums(a, m, cur_b);
@@ -1172,6 +1238,18 @@ int hg_conv1x1_blocked_bwd(const float* g, const float* g2, const float* aux, co
   a.act = act; a.ascale = ascale; a.rgb_w = rk_v ? rk_w : nullptr; a.rk_v = rk_v; a.rk_n = rk_n;
   return launch_blocked_gemm(a, passes, true, static_cast<cudaStream_t>(stream), "hg_conv1x1_blocked_bwd");
 }
+
+#ifdef HG_SPADE_PROFILE
+// nanoseconds per phase summed over the warpgroups of every const-style launch since the last read, then the count of
+// warpgroup-tiles; clears the sums
+int hg_spade_profile_read(unsigned long long* host) {
+  unsigned long long zero[hg::kProfPhases + 1] = {};
+  if (cudaMemcpyFromSymbol(host, hg::g_spade_prof, sizeof(zero)) != cudaSuccess ||
+      cudaMemcpyToSymbol(hg::g_spade_prof, zero, sizeof(zero)) != cudaSuccess)
+    return 1;
+  return 0;
+}
+#endif
 
 int hg_bn_finalize(const double* stats, double count, const double* count_dev, const float* weight, const float* bias, float* running_mean,
                    float* running_var, int training, float eps, float momentum, const float* gb, int B, int C,

@@ -108,6 +108,13 @@ __device__ __forceinline__ void lds8(uint32_t a, float (&o)[8]) {
   o[4] = y.x; o[5] = y.y; o[6] = y.z; o[7] = y.w;
 }
 
+// One fp32 entry of such a table (same contract as lds8).
+__device__ __forceinline__ float lds1(uint32_t a) {
+  float v;
+  asm("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a));
+  return v;
+}
+
 // ---------------------------------------------------------------- proxies / fences
 // generic-proxy writes (st.shared) -> visible to the async proxy (wgmma operand reads / bulk copies)
 __device__ __forceinline__ void fence_proxy_async_smem() {
